@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the Point-SAM hot path (BASELINE.json metric: point-clouds/sec, N=32768, ViT-L, 512x64 groups).
 
-  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--config c2] [--no-graph]
+  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--config c2] [--no-graph] [--dump-outputs DIR]
 
 Headline workload (config c2, BASELINE.json configs[1]): independent single-cloud requests (B=1, N=32768, G=512, K=64,
 EVA02-L, one point prompt) through FPS + kNN grouping + mini-PointNet + ViT-L encoder + prompt decoder -> mask logits.
@@ -17,6 +17,10 @@ The same line carries "c3" (BASELINE.json configs[2], run after the c2 arms unle
 sharded contiguously over the ranks (strong scaling), 3 prompt iterations of the evaluation loop
 (forward(is_eval=True): GT-driven prompt sampling, mask feedback) as CUDA graphs of 4 clouds, and the NCCL all_gather
 of the per-cloud IoU rows INSIDE the timed region.
+
+`--dump-outputs DIR` writes, after the timed steps, the arrays the callers of the timed path received in its last step
+(mask logits and IoU predictions of the clouds of that step still held by the lanes) as float32 .npy files; the inputs
+and weights are seeded, so two builds can be compared output for output.
 
 `--impl reference` times the reference's own algorithm on the host cores: the oracle port (oracle/tokenizer_ref.c FPS
 + oracle/torch_ref.py PyTorch fp32 path; the reference has no CPU FPS and timm is not installable offline, DESIGN.md).
@@ -56,10 +60,8 @@ METRIC = "point-clouds/sec (N=32768, ViT-L, 512x64 groups)"  # BASELINE.json met
 
 
 def peaks():
-    try:
-        return json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json"))), "measured"
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    """NVIDIA's data-sheet figures for the H100 SXM at 700 W (dense BF16, HBM3); a power-limited card reaches less."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -95,6 +97,24 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
+def dump_outputs(pp, cps: int, out_dir: str) -> dict:
+    """Mask logits [n, B, C, N] and IoU predictions [n, B, C] of the last timed step's tickets that are still held by the
+    lanes (the last min(cps, depth) tickets: each lane keeps its latest result), as float32 .npy files in out_dir."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    tickets = range(pp.count - min(cps, pp.depth), pp.count)
+    masks, iou = [], []
+    for t in tickets:
+        m, i = pp.result(t)
+        masks.append(m.float().cpu().numpy())
+        iou.append(i.float().cpu().numpy())
+    arrays = {"masks": np.stack(masks).astype(np.float32), "iou": np.stack(iou).astype(np.float32)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    return {"dir": out_dir, "tickets": [tickets.start, tickets.stop], **{k: list(a.shape) for k, a in arrays.items()}}
+
+
 def workload_config(args, name):
     """IDENTICAL on the repo arm and the reference arm (the driver compares the two `config` objects); everything
     specific to how one arm runs the workload goes into the line's "run" object instead."""
@@ -107,7 +127,7 @@ def workload_config(args, name):
         wl = (f"{name}: independent requests of {bpg} cloud(s), N={N}, group_number={G}, group_size={K}, {enc}, "
               f"{P} point prompt, multimask")
     return {"workload": wl, "parallelism": f"dp{args.gpus} (clouds sharded by rank, weights replicated)",
-            "l2": "inputs larger than L2: packed weights (1.3 GB for ViT-L) + activations exceed the 126 MB L2 and are "
+            "l2": "inputs larger than L2: packed weights (1.3 GB for ViT-L) + activations exceed the 50 MB L2 and are "
                   "re-streamed for every cloud; the input clouds rotate"}
 
 
@@ -165,8 +185,8 @@ def run_reference(args):
 
 
 def run_gpu_reference(args):
-    """Subprocess mode (`--impl gpu-reference`): SURVEY.md 8(d) "GPU reference beside it" - the reference's own GPU
-    execution model on this box (its FPS kernel compiled for sm_100a from oracle/_ref when it travelled + cdist/topk +
+    """Subprocess mode (`--impl gpu-reference`): "GPU reference beside it" - the reference's own GPU
+    execution model on the same GPU (its FPS kernel compiled for sm_90a from oracle/_ref when it was built + cdist/topk +
     PyTorch fp32 eager modules = the oracle restatement on cuda:0), plus full-size parity of the CUDA path against it on
     this very workload.  A reported comparison point only; nothing here is product code."""
     from oracle import build_ref, synth, torch_ref
@@ -450,6 +470,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true", help="skip the same-GPU PyTorch-eager reference timing")
     ap.add_argument("--no-roofline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -545,6 +567,8 @@ def main():
         sampler.start()  # samples clocks / throttle reasons over the warm-up and both timed arms
     timed(step_dev, args.warmup)
     ms_dev = timed(step_dev, args.steps)
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(pp, cps, args.dump_outputs)
 
     # single-stream latency of one cloud (no overlap between clouds), for the record
     n_single = max(3, min(24, args.steps))
@@ -591,6 +615,8 @@ def main():
                     "ms_per_step": ms_e2e / args.steps},
             "gpu_launches": pred.launches_per_step * cps * args.steps, "launches_per_cloud": pred.launches_per_step,
             "clocks": clocks, "mean_iou_pred": float(checksum)}
+    if args.dump_outputs and rank == 0:
+        line["dumped_outputs"] = dumped
 
     # ---- config c3 on the same ranks (the sharded workload: strong scaling, collective inside the timed region) ----
     if not args.no_c3 and args.config == "c2" and os.environ.get("PSAM_PROFILE_STAGE") is None:
@@ -607,7 +633,7 @@ def main():
         from psam_b200 import engine, ops
 
         pk, pk_src = peaks()
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+        peak = pk["bf16_tflops"]
         real = nv.lib()
         hint = 1 if pp.depth > 1 and pp.throughput_tiles else 0
 
@@ -651,17 +677,10 @@ def main():
         tot_serial = sum(s["ms"] for s in serial.values())
         ms_gemm, n_gemm, flops_cloud = only_regime(pp, ("psam_gemm_bf16x3",), reps=12)
         tf_regime, us_launch = flops_cloud / (ms_gemm / 1e3) / 1e12, ms_gemm * 1e3 / max(1, n_gemm)
-        traffic, traffic_src = None, None
-        for f in ("r02_gemm_traffic.json",):
-            try:
-                tj = json.load(open(os.path.join(REPO, "profiles", f)))
-                traffic, traffic_src = tj["dram_bytes_per_launch"], f"profiles/{f}: {tj.get('how', 'ncu --set full')}"
-            except Exception:
-                pass
         line["roofline"] = {
-            "bound": "tensor", "kernel": "gemm_tc_kernel (tcgen05 split-bf16)", "achieved": tf_regime, "peak": peak,
-            "unit": "TFLOP/s", "frac": tf_regime / peak, "traffic": traffic, "traffic_source": traffic_src,
-            "peak_source": f"{pk_src} sustained bf16",
+            "bound": "tensor", "kernel": "gemm_wgmma_kernel (split-bf16)", "achieved": tf_regime, "peak": peak,
+            "unit": "TFLOP/s", "frac": tf_regime / peak, "peak_source": f"{pk_src} dense bf16",
+            "device": torch.cuda.get_device_name(dev),
             "regime": f"the step's {n_gemm} GEMM launches (same tiles, epilogues, buffers as the timed graphs) replayed alone on "
                       f"{pp.depth} concurrent streams; achieved = algorithmic flops 2MNK / elapsed",
             "executed_tflops": 3 * tf_regime, "executed_frac": 3 * tf_regime / peak,
@@ -676,7 +695,7 @@ def main():
                           "note": f"lane 0 event-bracketed (throughput tiles) while the other {pp.depth - 1} lanes replay their graphs"},
             "serial": {"launches": gs["n"], "avg_launch_us": gs["ms"] / gs["n"] * 1e3, "sum_ms": gs["ms"],
                        "achieved": gs["flops"] / (gs["ms"] / 1e3) / 1e12, "share_of_serial_step": gs["ms"] / tot_serial,
-                       "note": "same tiles, lane 0 alone: one 48-CTA GEMM at a time cannot fill 148 SMs"},
+                       "note": "same tiles, lane 0 alone: one 48-CTA GEMM at a time cannot fill 132 SMs"},
             "note": "achieved counts the ALGORITHMIC fp32 flops 2MNK; the kernel executes 3 bf16 MMA passes per product (executed_* = x3)"}
         f = serial.get("psam_fps_f32")
         if f:
@@ -689,7 +708,7 @@ def main():
                                          "frac_of_hbm": fb / (ms_r / 1e3) / 1e9 / pk["hbm_gbs"],
                                          "note": f"FPS launches of {pp.depth} clouds in flight (the timed regime): one 8-CTA cluster per "
                                                  "cloud, the clusters of different clouds run side by side"},
-                           "note": "byte model (G-1)*N*20 B of SURVEY 8(d) = what the reference kernel streams; this kernel keeps the "
+                           "note": "byte model (G-1)*N*20 B = what the reference kernel streams; this kernel keeps the "
                                    "cloud in registers (real DRAM traffic = the cloud once) and is a latency chain: us_per_iter is the "
                                    "figure of merit for one cloud"}
         k = serial.get("psam_knn_f32")
@@ -707,7 +726,7 @@ def main():
             line["tokenizer_in_regime"] = {
                 "machine_ms_per_cloud": ms_r, "byte_model_gbs": (fb + kb) / (ms_r / 1e3) / 1e9,
                 "frac_of_hbm": (fb + kb) / (ms_r / 1e3) / 1e9 / pk["hbm_gbs"], "hbm_peak_gbs": pk["hbm_gbs"],
-                "note": f"the FPS + kNN launches of {pp.depth} clouds in flight replayed alone (the timed regime); bytes = SURVEY 8(d) "
+                "note": f"the FPS + kNN launches of {pp.depth} clouds in flight replayed alone (the timed regime); bytes = "
                         "byte models (FPS streaming model + kNN reference-equivalent), not DRAM traffic"}
         at = serial.get("psam_attention_bf16x3")
         if at:
@@ -719,7 +738,7 @@ def main():
             line["attention"] = {"us_per_layer": at["ms"] / at["n"] * 1e3, "layers": at["n"],
                                  "algorithmic_tflops": aflops / (at["ms"] / at["n"] / 1e3) / 1e12,
                                  "executed_frac_of_peak": 3 * aflops / (at["ms"] / at["n"] / 1e3) / 1e12 / peak,
-                                 "note": "serial, lone launch; tensor-pipe % of the kernel is in profiles/ (ncu)"}
+                                 "note": "serial, lone launch"}
         line["stage_ms_serial"] = {n: round(s["ms"], 4) for n, s in sorted(serial.items(), key=lambda kv: -kv[1]["ms"])}
 
     if rank == 0:

@@ -1,4 +1,4 @@
-/* psam_b200 - C ABI of the B200-native Point-SAM hot path.
+/* psam_b200 - C ABI of the Point-SAM hot path on the H100 (sm_90a).
  *
  * This is the drop-in boundary.  In the reference the native boundary for this path is the pybind11
  * module torkit3d._C (third_party/torkit3d/torkit3d/csrc/torkit3d.cpp:10-23,
@@ -124,7 +124,8 @@ typedef struct {
     int act;                /* PSAM_ACT_* applied after bias/residual */
     int accumulate;         /* 1: out_f32 += alpha*acc (+bias) with red.add; required when split_k>1 */
     int swiglu;             /* 1: W rows interleaved (gate_i, value_i); out_f32[:, i] = silu(gate_i)*value_i (fp32 out only) */
-    int tile_hint;          /* 0: tile width for lowest latency; 1: for lowest SM-time (several clouds in flight); 32..256: explicit */
+    int tile_hint;          /* 0: tile width for lowest latency; 1: for lowest SM-time (several clouds in flight); 32..256: explicit
+                               (a multiple of 32, rounded up to the tile widths the kernel has: 64, 128, 256) */
     float* gmax;            /* optional fused max-pool: gmax[(row / group_rows) * ld_gmax + col] = max over the group rows
                                (atomic; caller pre-fills with -inf; group_rows multiple of 32); replaces torch.max(x, dim=-2) */
     long long ld_gmax;
@@ -145,16 +146,11 @@ typedef struct {
     const float* ln_c;
     int ln_h;
     float ln_eps;
-    int variant;            /* 0 = policy default.  Experiment switches (the library reads no environment variable):
-                             * 0x1 cta_group::2 pairs, 0x2 BK=32 4-stage ring, 0x4 scalar epilogue, 0x8 the dual-resident
-                             * wide-tile kernel (two 97 KB CTAs per SM; 0x10 overrides it),
-                             * 0x80 two MMA-issuing warps for wide one-shot tiles (measured no gain: opt-in),
-                             * 0x20 force / 0x40 forbid the persistent kernel (tile loop inside the CTA, double-buffered TMEM
-                             * accumulator; default when the launch has >= 2 tiles per SM), bits 16-19 tiles per CTA to aim for,
-                             * bits 8-11 W-tile multicast cluster size (2|4), bits 12-15 L2 prefetch depth in k-blocks */
+    int variant;            /* 0 = policy default.  0x4 forces the scalar epilogue (the library reads no environment
+                             * variable); every other bit is accepted and has no effect on sm_90a */
 } psam_gemm_out;
 
-/* C[M,N] = A[M,K] * W[N,K]^T on tcgen05 tensor cores (TMA-fed, TMEM accumulators).
+/* C[M,N] = A[M,K] * W[N,K]^T on the tensor cores (TMA-fed wgmma, fp32 register accumulators).
  * passes=3: split-bf16 emulation of the reference's fp32 nn.Linear / bmm; passes=1: hi planes only.
  * Replaces nn.Linear / F.linear / @ on the PatchEncoder, ViT blocks and upscaling MLP
  * (common.py:486-497, pc_encoder.py:99-116,136-143, timm EvaBlock, mask_decoder.py:53-59). */
@@ -163,7 +159,7 @@ int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, const psam_ge
 
 /* Row-complete GEMM with LayerNorm and activation in the epilogue:
  *   Y = act(LayerNorm(A W^T + gbias[row / group_rows])) as split-bf16, A [M,K<=128], W [N,K] with N = 256 or 512 (a CTA owns
- * 128 rows x the full width, so the row statistics stay on the SM and the fp32 pre-activation never reaches memory).
+ * 128 rows x the full width, so the row statistics stay in registers and the fp32 pre-activation never reaches memory).
  * Replaces conv2[0..2] of PatchEncoder (Linear on cat[max, x] = W_a max + W_b x, LayerNorm, GELU; common.py:491-495):
  * gbias carries W_a max + b per group.  gamma / beta [N]; out_hi [M, ldo_s] hi plane, lo plane out_plane elements further. */
 int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand* w, const float* gbias, long long ld_gbias, int group_rows,
@@ -174,17 +170,15 @@ int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand* w, const f
  * q/k/v are split-bf16 operand views [L rows x dh] with nb1 = heads, nb2 = clouds (typically three column windows of
  * the fused qkv activation).  dh == 64 or 88 (EVA-giant; the 88-wide head is handled as 64 + 24 columns, zero padded by
  * TMA), any L >= 1 (PSAM_ERR_UNSUPPORTED otherwise - the caller then uses
- * psam_gemm_bf16x3 + psam_softmax_split).  Key blocks are streamed once: S_j lands in a ring of tensor-memory slots,
- * P_j = exp2(S_j c - m_ref) is written back into the slot as split-bf16 and consumed as the TMEM A operand of the PV
- * MMA; the reference maximum is moved (and O rescaled) only when a block exceeds it by more than 2^8.
+ * psam_gemm_bf16x3 + psam_softmax_split).  Key blocks are streamed once: S_j = Q K_j^T stays in registers, the running row
+ * maximum rescales O and the row sum when it grows, and P_j (split-bf16, in registers) is the A operand of the PV wgmma.
  * Replaces F.scaled_dot_product_attention in timm EvaAttention (blocks called at pc_encoder.py:138-139). */
 int psam_attention_bf16x3(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi,
                           long long out_plane, long long ldo, long long out_head_stride, long long out_cloud_stride,
                           float scale, cudaStream_t stream);
 
-/* Same contract, computed by the first-generation kernels (exact two-pass softmax with S resident in tensor memory for
- * L <= 512, two-sweep ring for longer rows, P staged through shared memory).  Kept as an independent implementation
- * the tests cross-check the streaming kernel against. */
+/* Same contract for dh == 64, with an exact two-pass softmax: a first sweep over the key blocks computes the row maximum,
+ * the second exponentiates with it (nothing is rescaled).  The tests cross-check the streaming form against it. */
 int psam_attention_bf16x3_twopass(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi,
                                   long long out_plane, long long ldo, long long out_head_stride,
                                   long long out_cloud_stride, float scale, cudaStream_t stream);

@@ -1,7 +1,8 @@
-"""ORACLE tooling (NOT product code): compile the REFERENCE's own CUDA kernels for sm_100a, from the
-sources where they lie under /root/reference (nothing is copied), into oracle/_ref/ (git-ignored, travels
-to the GPU box).  Used by the GPU tests to pin FPS bit-exactness (incl. the tie-break rule) and the
-nearest-neighbour distance against the real reference kernels.
+"""ORACLE tooling (NOT product code): compile the REFERENCE's own CUDA kernels for sm_90a, from the
+sources where they lie in a checkout of the reference named by PSAM_REFERENCE (nothing is
+copied), into oracle/_ref/ (git-ignored).  oracle/make_ref_golden.py runs them once on a GPU and stores their
+outputs under tests/golden/, which the GPU tests compare against (FPS bit-exactness incl. the tie-break rule,
+nearest-neighbour distance).
 
 Sources compiled: third_party/torkit3d/torkit3d/csrc/cuda/{sample_farthest_points,chamfer_distance}_kernel.cu
 with a 10-line pybind shim (oracle/ref_binding.cpp) - the reference's setup.py is not run.
@@ -13,7 +14,7 @@ import shutil
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/third_party/torkit3d/torkit3d/csrc"
+REF = os.path.join(os.environ.get("PSAM_REFERENCE", ""), "third_party", "torkit3d", "torkit3d", "csrc")
 OUT = os.path.join(HERE, "_ref")
 NAME = "torkit3d_ref_ops"
 
@@ -30,10 +31,10 @@ def built_path():
 def build(verbose=False):
     if built_path():
         return built_path()
-    if not os.path.isdir(REF):
+    if not os.environ.get("PSAM_REFERENCE") or not os.path.isdir(REF):
         return None
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     from torch.utils.cpp_extension import load
 
     load(name=NAME,
@@ -41,7 +42,7 @@ def build(verbose=False):
                   os.path.join(REF, "cuda", "sample_farthest_points_kernel.cu"),
                   os.path.join(REF, "cuda", "chamfer_distance_kernel.cu")],
          extra_include_paths=[os.path.join(REF, "include")],
-         extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a", "-O3"],
+         extra_cuda_cflags=["-gencode", "arch=compute_90a,code=sm_90a", "-O3"],
          build_directory=OUT, verbose=verbose, is_python_module=False)
     for f in os.listdir(OUT):  # keep only the shared object
         if not f.endswith(".so"):
@@ -51,7 +52,7 @@ def build(verbose=False):
 
 
 def load_ref():
-    """Import the compiled reference ops (GPU box: uses the prebuilt .so that travelled with the repo)."""
+    """Import the compiled reference ops (None where oracle/_ref was not built)."""
     p = built_path()
     if p is None:
         return None

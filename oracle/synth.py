@@ -1,4 +1,4 @@
-"""Deterministic synthetic inputs (SURVEY.md section 8d).  The generator lives with the product package
+"""Deterministic synthetic inputs.  The generator lives with the product package
 (psam_b200/synth.py) so that bench.py's repo arm never imports anything under oracle/; the oracle-side tests and the
 golden-vector generator use it through this re-export."""
 import os

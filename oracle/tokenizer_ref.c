@@ -8,8 +8,8 @@
  *                        (per-thread strided scan :45-73, shared-memory tree :82-95, block size from
  *                        csrc/include/utils.h:13-19 capped at 512 with a floor of 32, :132-161).
  *                        Squared distance is fmaf(dz,dz,fmaf(dy,dy,dx*dx)) with d = p_j - p_sel, the
- *                        contraction nvcc emits for the loop at :51-55 (SASS-verified, SURVEY.md).
- *  oracle_fps_closed_f32 the closed form of the same tie-break (SURVEY.md section 8 a-1): among the
+ *                        contraction nvcc emits for the loop at :51-55 (SASS-verified).
+ *  oracle_fps_closed_f32 the closed form of the same tie-break: among the
  *                        points holding the maximum min-distance pick the lexicographic minimum of
  *                        (bitrev(j mod T), j div T); repeat the previous index when the maximum is 0.
  *  oracle_knn_f32        exact brute-force K nearest (direct-difference squared distance, ties broken

@@ -20,10 +20,10 @@ state-dict key names so that weights can be exchanged with ``load_state_dict``:
                         timm/models/eva.py EvaAttention / EvaBlock / Eva and timm/layers/mlp.py
                         SwiGLU / Mlp, restated from the published source.  PARITY UNPINNED for this
                         part: timm is not installable offline and the reference holds no test or
-                        golden vector at this boundary (SURVEY.md section 8c).
+                        golden vector at this boundary.
 
 Distance semantics: the reference's ``torch.cdist`` uses the matmul expansion whose rounding noise
-differs between backends (SURVEY.md section 7, hard part 3).  ``exact_dist=True`` (default) uses the
+differs between backends.  ``exact_dist=True`` (default) uses the
 direct-difference form ``compute_mode="donot_use_mm_for_euclid_dist"`` which is what the CUDA path
 implements; ``exact_dist=False`` reproduces the reference call literally.
 """

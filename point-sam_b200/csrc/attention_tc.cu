@@ -1,20 +1,23 @@
-// Fused multi-head self-attention for sm_100a (encoder blocks): O = softmax(Q K^T * scale) V.
+// Fused multi-head self-attention for sm_90a (encoder blocks): O = softmax(Q K^T * scale) V.
 //
 // Replaces F.scaled_dot_product_attention inside timm's EvaAttention (called from
 // pc_sam/model/pc_encoder.py:138-139 via block(x); rope=None, no mask) and the four unfused kernels of
-// the first implementation (QK^T GEMM, softmax, V transpose, PV GEMM).
+// an unfused implementation (QK^T GEMM, softmax, V transpose, PV GEMM).
 //
-// One CTA per (cloud, head, 128-query tile).  All key blocks of the row fit the tensor memory
-// (L <= 512 keys -> S is 128 x 512 fp32 = the full 512 TMEM columns), so softmax is EXACT two-pass
-// (row max over all keys, then exp) - no online rescaling:
-//   warp 0    TMA producer: Q tile once, then K blocks, then V blocks through a 3-stage ring
-//             (each stage = one 128-row x 64 block, hi+lo planes, 32 KB)
-//   warp 1    MMA issuer: S_j = Q K_j^T (split-bf16, 3 passes) into TMEM columns [128j,128j+128);
-//             later O += P_j V_j with P from shared memory (K-major) and V^T taken directly from the
-//             row-major V block as an MN-major B operand (no transpose pass); O reuses columns [0,64)
-//   warps 2-9 softmax: two threads per query row (each owns every other 32-key group); tcgen05.ld S, row
-//             max, ex2.approx, split P into bf16 hi/lo and write it 128B-swizzled into shared memory for
-//             the PV MMA; finally O / rowsum -> split-bf16
+// One CTA per (cloud, head, 128-query tile); two consumer warpgroups of 64 query rows each and one TMA warp.
+//   warp 8     TMA producer: the Q tile once, then 64-key K and V blocks through a 4-stage mbarrier ring
+//              (each stage = one 64-row block, hi+lo planes, per 64-column chunk of the head)
+//   warps 0-7  per warpgroup and key block j:
+//                S_j = Q K_j^T with wgmma (split-bf16, 3 passes) into fp32 registers,
+//                softmax in registers (the four lanes of a quad share a row),
+//                P_j split into bf16 hi/lo registers that are DIRECTLY the A operand of the next wgmma (the accumulator
+//                fragment of m64n64 is the A fragment of k16 steps), O += P_j V_j with V_j^T read from the row-major V
+//                block as an MN-major shared-memory B operand (no transpose pass)
+// Streaming form (psam_attention_bf16x3): running row maximum, O and the row sum rescaled when it grows.
+// Two-pass form (psam_attention_bf16x3_twopass, dh = 64): a first sweep over the K blocks computes the exact row maximum;
+// the second sweep exponentiates with it, so nothing is rescaled.
+// Head dims 64 and 88 (EVA-giant): dh = 88 is loaded as two 64-column chunks, the second holding columns 64..87 and the
+// zeros TMA fills in beyond the head's extent.
 // Numerics follow the split-bf16 scheme of gemm_tc.cu (x ~= hi + lo, three MMA passes).
 #include "psam_common.cuh"
 #include "../../include/psam_b200.h"
@@ -22,610 +25,25 @@
 namespace psam {
 
 constexpr int ATT_BQ = 128;        // queries per CTA
-constexpr int ATT_BKEY = 128;      // keys per block
-constexpr int ATT_DH = 64;         // head dim handled by this kernel
-constexpr int ATT_STAGES = 3;
-constexpr int ATT_THREADS = 320;  // TMA warp, MMA warp, 8 softmax warps (2 threads per query row)
-constexpr int ATT_TILE = 128 * 64 * 2;                 // one 128x64 bf16 tile (one plane)
-constexpr int ATT_SMEM_Q = 2 * ATT_TILE;               // hi + lo
-constexpr int ATT_SMEM_STAGE = 2 * ATT_TILE;           // hi + lo of a K or V block
-constexpr int ATT_SMEM_P = 2 * 2 * ATT_TILE;           // hi + lo, 2 k-blocks of 64 keys
-constexpr int ATT_SMEM_TOTAL = ATT_SMEM_Q + ATT_STAGES * ATT_SMEM_STAGE + ATT_SMEM_P + 1024 /*row exchange*/ + 1024 /*alignment*/;
+constexpr int ATT_BKEY = 64;       // keys per block
+constexpr int ATT_STAGES = 4;
+constexpr int ATT_THREADS = 288;   // two consumer warpgroups + one TMA warp
+constexpr int ATT_Q_TILE = 128 * 64 * 2;   // one plane of a 64-column chunk of the Q tile
+constexpr int ATT_KV_TILE = 64 * 64 * 2;   // one plane of a 64-column chunk of a K or V block
 
-// MN-major (N contiguous), 128B-swizzled B operand: rows of the tile are K (keys), 64 N-elements = 128 B per
-// row, 8-row swizzle atoms 1024 B apart along K.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(16384 >> 4) << 16;  // leading byte offset: next 64-wide N atom (unused, N = 64)
-    d |= (uint64_t)(1024 >> 4) << 32;   // stride byte offset: next 8-row group along K
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
+template <int NCH>
+struct AttSmem {
+    static constexpr int Q = NCH * 2 * ATT_Q_TILE;
+    static constexpr int STAGE = NCH * 2 * ATT_KV_TILE;
+    static constexpr int TOTAL = Q + ATT_STAGES * STAGE + 1024;
+};
 
 struct AttnParams {
     int L, H, B;
     float scale_log2e;  // softmax scale * log2(e)
     __nv_bfloat16* out_hi;
     long long out_plane, ldo, out_h, out_b;  // elements: plane offset, row stride, head / cloud strides
-    unsigned long long* trace;               // debug timeline (tools/attention_trace.py): null in production
-    int tiles_per_cta;                       // attention_pair_kernel: 1 or 2 query tiles per CTA
 };
-
-__device__ __forceinline__ void att_trace(const AttnParams& p, int slot) {
-    // one 64-bit clock stamp per (CTA, slot); only CTA (0,0,0) records, one lane per call site
-    if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%clock64;" : "=l"(t));
-        p.trace[slot] = t;
-    }
-}
-
-__global__ void __launch_bounds__(ATT_THREADS, 1)
-attention_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                    const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
-    pdl_launch_dependents();
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t q_full, s_full, p_full, p_empty, o_full;
-    __shared__ __align__(8) uint64_t kv_full[ATT_STAGES], kv_empty[ATT_STAGES];
-    __shared__ uint32_t tmem_base_smem;
-
-    const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    const uint32_t sQ = smem_base;
-    const uint32_t sKV = sQ + ATT_SMEM_Q;
-    const uint32_t sP = sKV + ATT_STAGES * ATT_SMEM_STAGE;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q_tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int nkb = (p.L + ATT_BKEY - 1) / ATT_BKEY;  // key blocks (<= 4)
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_q);
-        tma_prefetch_desc(&tmap_k);
-        tma_prefetch_desc(&tmap_v);
-        mbar_init(smem_u32(&q_full), 1);
-        mbar_init(smem_u32(&s_full), 1);
-        mbar_init(smem_u32(&p_full), 256);
-        mbar_init(smem_u32(&p_empty), 1);
-        mbar_init(smem_u32(&o_full), 1);
-        for (int s = 0; s < ATT_STAGES; ++s) {
-            mbar_init(smem_u32(&kv_full[s]), 1);
-            mbar_init(smem_u32(&kv_empty[s]), 1);
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    pdl_wait();  // everything above is independent of the previous kernel; its outputs are read only below
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            const uint32_t qb = smem_u32(&q_full);
-            mbar_arrive_expect_tx(qb, ATT_SMEM_Q);
-            tma_load_5d(sQ, &tmap_q, qb, 0, q_tile * ATT_BQ, 0, h, b);  // one 3-D box: hi plane then lo plane
-            for (int i = 0; i < 2 * nkb; ++i) {  // K blocks then V blocks
-                const int s = i % ATT_STAGES;
-                const uint32_t ph = (uint32_t)(i / ATT_STAGES) & 1u;
-                mbar_wait(smem_u32(&kv_empty[s]), ph ^ 1u);
-                const uint32_t fb = smem_u32(&kv_full[s]);
-                mbar_arrive_expect_tx(fb, ATT_SMEM_STAGE);
-                const CUtensorMap* tm = (i < nkb) ? &tmap_k : &tmap_v;
-                const int j = (i < nkb) ? i : i - nkb;
-                tma_load_5d(sKV + s * ATT_SMEM_STAGE, tm, fb, 0, j * ATT_BKEY, 0, h, b);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        constexpr uint32_t idesc_s = umma_idesc_bf16(128, ATT_BKEY);                   // S: A,B K-major
-        constexpr uint32_t idesc_o = umma_idesc_bf16(128, ATT_DH) | (1u << 16);        // O: B (V) MN-major
-        mbar_wait(smem_u32(&q_full), 0);
-        tc_fence_after();
-        const uint64_t q_hi = umma_desc_k_sw128(sQ), q_lo = umma_desc_k_sw128(sQ + ATT_TILE);
-        for (int j = 0; j < nkb; ++j) {
-            const int i = j, s = i % ATT_STAGES;
-            mbar_wait(smem_u32(&kv_full[s]), (uint32_t)(i / ATT_STAGES) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sk = sKV + s * ATT_SMEM_STAGE;
-                const uint64_t k_hi = umma_desc_k_sw128(sk), k_lo = umma_desc_k_sw128(sk + ATT_TILE);
-                const uint32_t d_s = tmem_base + (uint32_t)(j * ATT_BKEY);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_hi + 2 * k, k_hi + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_lo + 2 * k, k_hi + 2 * k, idesc_s, 1u);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_hi + 2 * k, k_lo + 2 * k, idesc_s, 1u);
-                umma_commit(smem_u32(&kv_empty[s]));
-                if (j == nkb - 1) umma_commit(smem_u32(&s_full));
-            }
-            __syncwarp();
-        }
-        const uint64_t p_hi = umma_desc_k_sw128(sP), p_lo = umma_desc_k_sw128(sP + 2 * ATT_TILE);
-        for (int j = 0; j < nkb; ++j) {
-            const int i = nkb + j, s = i % ATT_STAGES;
-            mbar_wait(smem_u32(&kv_full[s]), (uint32_t)(i / ATT_STAGES) & 1u);
-            mbar_wait(smem_u32(&p_full), (uint32_t)j & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sv = sKV + s * ATT_SMEM_STAGE;
-                const uint64_t v_hi = umma_desc_mn_sw128(sv), v_lo = umma_desc_mn_sw128(sv + ATT_TILE);
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    // P: k-block (ks/4) of 64 keys is 16 KB further, 32 B per 16-key step inside it; V: 16 rows = 2048 B
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_hi + pa, v_hi + va, idesc_o, (j > 0 || ks > 0) ? 1u : 0u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_lo + pa, v_hi + va, idesc_o, 1u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_hi + pa, v_lo + va, idesc_o, 1u);
-                }
-                umma_commit(smem_u32(&kv_empty[s]));
-                umma_commit(smem_u32(&p_empty));
-                if (j == nkb - 1) umma_commit(smem_u32(&o_full));
-            }
-            __syncwarp();
-        }
-    } else {
-        // ===================== softmax / epilogue warps (2 threads per query row) =====================
-        const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-        const int sub = (warp - 2) >> 2;          // 0/1: which half of the 32-column groups this thread owns
-        const int r = quarter * 32 + lane;        // row inside the tile == TMEM lane
-        const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        float* xchg = reinterpret_cast<float*>(smem_dyn + (smem_base - smem_u32(smem_dyn)) + ATT_SMEM_Q + ATT_STAGES * ATT_SMEM_STAGE +
-                                               ATT_SMEM_P);  // 2 x 128 floats, after the P buffer
-        mbar_wait(smem_u32(&s_full), 0);
-        tc_fence_after();
-        // ---- pass A: row maximum over all keys (each thread scans its half, halves combined through smem) ----
-        float mx = -3.0e38f;
-        for (int g = sub; g < nkb * (ATT_BKEY / 32); g += 2) {
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)(g * 32), v);
-            tmem_ld_wait();
-            const int key0 = g * 32;
-            if (key0 + 32 <= p.L) {
-#pragma unroll
-                for (int t = 0; t < 32; ++t) mx = fmaxf(mx, __uint_as_float(v[t]));
-            } else {
-#pragma unroll
-                for (int t = 0; t < 32; ++t)
-                    if (key0 + t < p.L) mx = fmaxf(mx, __uint_as_float(v[t]));
-            }
-        }
-        xchg[sub * 128 + r] = mx;
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // the 8 softmax warps only
-        mx = fmaxf(mx, xchg[(sub ^ 1) * 128 + r]);
-        const float mscaled = mx * p.scale_log2e;
-        // ---- pass B: P_j = exp2(s*scale*log2e - m) -> shared memory, partial row sum --------------------
-        float lsum = 0.f;
-        for (int j = 0; j < nkb; ++j) {
-            if (j > 0) mbar_wait(smem_u32(&p_empty), (uint32_t)(j - 1) & 1u);  // PV_{j-1} has consumed P
-#pragma unroll 1
-            for (int c = sub; c < ATT_BKEY / 32; c += 2) {
-                uint32_t v[32];
-                tmem_ld_32x32(t_row + (uint32_t)(j * ATT_BKEY + c * 32), v);
-                tmem_ld_wait();
-                const int key0 = j * ATT_BKEY + c * 32;
-                const bool full = key0 + 32 <= p.L;
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int t = 0; t < 32; t += 2) {
-                    float e0, e1;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(__uint_as_float(v[t]), p.scale_log2e, -mscaled)));
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(__uint_as_float(v[t + 1]), p.scale_log2e, -mscaled)));
-                    if (!full) {
-                        if (key0 + t >= p.L) e0 = 0.f;
-                        if (key0 + t + 1 >= p.L) e1 = 0.f;
-                    }
-                    lsum += e0 + e1;
-                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(e0, e1);
-                    const float2 hf = __bfloat1622float2(h2);
-                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(e0 - hf.x, e1 - hf.y);
-                    hi[t >> 1] = *reinterpret_cast<const uint32_t*>(&h2);
-                    lo[t >> 1] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-                // keys [c*32, c*32+32) of this block: k-block kb = c/2, 16-byte chunks (c&1)*4 .. +3 of row r
-                const uint32_t rowbase = (uint32_t)((c >> 1) * ATT_TILE + r * 128);
-#pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {
-                    const uint32_t chunk = (uint32_t)(((c & 1) * 4 + q4) ^ (r & 7));
-                    st_shared_v4(sP + rowbase + chunk * 16, hi[q4 * 4], hi[q4 * 4 + 1], hi[q4 * 4 + 2], hi[q4 * 4 + 3]);
-                    st_shared_v4(sP + 2 * ATT_TILE + rowbase + chunk * 16, lo[q4 * 4], lo[q4 * 4 + 1], lo[q4 * 4 + 2], lo[q4 * 4 + 3]);
-                }
-            }
-            tc_fence_before();      // our TMEM reads of S_j are complete before the MMA may overwrite columns
-            fence_proxy_async();    // generic-proxy smem writes -> visible to the async proxy (UMMA)
-            mbar_arrive(smem_u32(&p_full));
-        }
-        // ---- epilogue: O / rowsum -> split-bf16 [B*L, H*dh]; thread `sub` stores 32 of the 64 columns ----
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // pass-A exchange values have been consumed by everyone
-        xchg[sub * 128 + r] = lsum;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        lsum += xchg[(sub ^ 1) * 128 + r];
-        mbar_wait(smem_u32(&o_full), 0);
-        tc_fence_after();
-        const int qrow = q_tile * ATT_BQ + r;
-        const float inv = 1.0f / lsum;
-        __nv_bfloat16* ohi = p.out_hi + (long long)b * p.out_b + (long long)h * p.out_h + (long long)qrow * p.ldo;
-        __nv_bfloat16* olo = ohi + p.out_plane;
-        {
-            const int c = sub;  // ATT_DH / 32 == 2 column groups
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)(c * 32), v);
-            tmem_ld_wait();
-            if (qrow < p.L) {
-#pragma unroll
-                for (int t = 0; t < 32; t += 8) {
-                    uint32_t hh[4], ll[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        __nv_bfloat16 h0, l0, h1, l1;
-                        split_bf16(__uint_as_float(v[t + 2 * u]) * inv, h0, l0);
-                        split_bf16(__uint_as_float(v[t + 2 * u + 1]) * inv, h1, l1);
-                        hh[u] = pack_bf16x2(h0, h1);
-                        ll[u] = pack_bf16x2(l0, l1);
-                    }
-                    *reinterpret_cast<uint4*>(ohi + c * 32 + t) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-                    *reinterpret_cast<uint4*>(olo + c * 32 + t) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-                }
-            }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------
-// Long sequences (L > 512: the reference evaluation runs group_number = 2048, evaluation/eval_kitti.py:352-362).
-// S no longer fits the tensor memory, so the row is swept twice over 128-key blocks, still with an EXACT softmax:
-//   sweep 1: S_j = Q K_j^T -> running row maximum only (no exponentials, no P, no PV)
-//   sweep 2: S_j recomputed -> P_j = exp2(S_j * c - m * c) with the final maximum -> O += P_j V_j, row sum
-// (1.5x the tensor work of one-sweep attention, no rescaling of O and no second exponential pass).
-// TMEM: O in columns [0,64); a ring of three 128-column S slots at columns 128/256/384, so the tensor pipe runs up to two
-// key blocks ahead of the softmax warps.  Shared memory and the warp roles are those of attention_tc_kernel.
-constexpr int ATT_SLOTS = 3;
-
-__global__ void __launch_bounds__(ATT_THREADS, 1)
-attention_tc_long_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                         const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t q_full, p_full, p_empty, o_full;
-    __shared__ __align__(8) uint64_t kv_full[ATT_STAGES], kv_empty[ATT_STAGES];
-    __shared__ __align__(8) uint64_t s_full[ATT_SLOTS], s_empty[ATT_SLOTS];
-    __shared__ uint32_t tmem_base_smem;
-
-    const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    const uint32_t sQ = smem_base;
-    const uint32_t sKV = sQ + ATT_SMEM_Q;
-    const uint32_t sP = sKV + ATT_STAGES * ATT_SMEM_STAGE;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q_tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-    const int nkb = (p.L + ATT_BKEY - 1) / ATT_BKEY;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_q);
-        tma_prefetch_desc(&tmap_k);
-        tma_prefetch_desc(&tmap_v);
-        mbar_init(smem_u32(&q_full), 1);
-        mbar_init(smem_u32(&p_full), 256);
-        mbar_init(smem_u32(&p_empty), 1);
-        mbar_init(smem_u32(&o_full), 1);
-        for (int s = 0; s < ATT_STAGES; ++s) {
-            mbar_init(smem_u32(&kv_full[s]), 1);
-            mbar_init(smem_u32(&kv_empty[s]), 1);
-        }
-        for (int s = 0; s < ATT_SLOTS; ++s) {
-            mbar_init(smem_u32(&s_full[s]), 1);
-            mbar_init(smem_u32(&s_empty[s]), 256);
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-
-    // Order in which the stage ring carries the operand blocks; the MMA warp consumes them in exactly this order:
-    //   K_0 .. K_{nkb-1}                                   (sweep 1)
-    //   K_0, K_1, then (K_{j+2}, V_j) for j = 0 .. nkb-1    (sweep 2; K runs two blocks ahead of V)
-    if (warp == 0) {
-        if (lane == 0) {
-            const uint32_t qb = smem_u32(&q_full);
-            mbar_arrive_expect_tx(qb, ATT_SMEM_Q);
-            tma_load_5d(sQ, &tmap_q, qb, 0, q_tile * ATT_BQ, 0, h, b);
-            int i = 0;
-            auto load = [&](const CUtensorMap* tm, int blk) {
-                const int s = i % ATT_STAGES;
-                mbar_wait(smem_u32(&kv_empty[s]), ((uint32_t)(i / ATT_STAGES) & 1u) ^ 1u);
-                const uint32_t fb = smem_u32(&kv_full[s]);
-                mbar_arrive_expect_tx(fb, ATT_SMEM_STAGE);
-                tma_load_5d(sKV + s * ATT_SMEM_STAGE, tm, fb, 0, blk * ATT_BKEY, 0, h, b);
-                ++i;
-            };
-            for (int j = 0; j < nkb; ++j) load(&tmap_k, j);
-            load(&tmap_k, 0);
-            if (nkb > 1) load(&tmap_k, 1);
-            for (int j = 0; j < nkb; ++j) {
-                if (j + 2 < nkb) load(&tmap_k, j + 2);
-                load(&tmap_v, j);
-            }
-        }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc_s = umma_idesc_bf16(128, ATT_BKEY);
-        constexpr uint32_t idesc_o = umma_idesc_bf16(128, ATT_DH) | (1u << 16);
-        mbar_wait(smem_u32(&q_full), 0);
-        tc_fence_after();
-        const uint64_t q_hi = umma_desc_k_sw128(sQ), q_lo = umma_desc_k_sw128(sQ + ATT_TILE);
-        const uint64_t p_hi = umma_desc_k_sw128(sP), p_lo = umma_desc_k_sw128(sP + 2 * ATT_TILE);
-        int i = 0;  // stage-ring item counter (same sequence as the producer)
-        auto issue_s = [&](int g) {  // S block number g (0 .. 2*nkb-1) into slot g % 3
-            const int s = i % ATT_STAGES, slot = g % ATT_SLOTS;
-            mbar_wait(smem_u32(&kv_full[s]), (uint32_t)(i / ATT_STAGES) & 1u);
-            if (g >= ATT_SLOTS) mbar_wait(smem_u32(&s_empty[slot]), (uint32_t)(g / ATT_SLOTS - 1) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sk = sKV + s * ATT_SMEM_STAGE;
-                const uint64_t k_hi = umma_desc_k_sw128(sk), k_lo = umma_desc_k_sw128(sk + ATT_TILE);
-                const uint32_t d_s = tmem_base + 128u + (uint32_t)(slot * ATT_BKEY);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_hi + 2 * k, k_hi + 2 * k, idesc_s, k > 0 ? 1u : 0u);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_lo + 2 * k, k_hi + 2 * k, idesc_s, 1u);
-#pragma unroll
-                for (int k = 0; k < ATT_DH / 16; ++k) umma_bf16(d_s, q_hi + 2 * k, k_lo + 2 * k, idesc_s, 1u);
-                umma_commit(smem_u32(&kv_empty[s]));
-                umma_commit(smem_u32(&s_full[slot]));
-            }
-            __syncwarp();
-            ++i;
-        };
-        for (int g = 0; g < nkb; ++g) issue_s(g);
-        issue_s(nkb);
-        if (nkb > 1) issue_s(nkb + 1);
-        for (int j = 0; j < nkb; ++j) {
-            if (j + 2 < nkb) issue_s(nkb + j + 2);
-            const int s = i % ATT_STAGES;
-            mbar_wait(smem_u32(&kv_full[s]), (uint32_t)(i / ATT_STAGES) & 1u);
-            mbar_wait(smem_u32(&p_full), (uint32_t)j & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sv = sKV + s * ATT_SMEM_STAGE;
-                const uint64_t v_hi = umma_desc_mn_sw128(sv), v_lo = umma_desc_mn_sw128(sv + ATT_TILE);
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_hi + pa, v_hi + va, idesc_o, (j > 0 || ks > 0) ? 1u : 0u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_lo + pa, v_hi + va, idesc_o, 1u);
-                }
-#pragma unroll
-                for (int ks = 0; ks < ATT_BKEY / 16; ++ks) {
-                    const uint64_t pa = (uint64_t)((ks >> 2) * (ATT_TILE >> 4) + (ks & 3) * 2);
-                    const uint64_t va = (uint64_t)(ks * (2048 >> 4));
-                    umma_bf16(tmem_base, p_hi + pa, v_lo + va, idesc_o, 1u);
-                }
-                umma_commit(smem_u32(&kv_empty[s]));
-                umma_commit(smem_u32(&p_empty));
-                if (j == nkb - 1) umma_commit(smem_u32(&o_full));
-            }
-            __syncwarp();
-            ++i;
-        }
-    } else {
-        const int quarter = warp & 3;
-        const int sub = (warp - 2) >> 2;
-        const int r = quarter * 32 + lane;
-        const uint32_t t_row = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        float* xchg = reinterpret_cast<float*>(smem_dyn + (smem_base - smem_u32(smem_dyn)) + ATT_SMEM_Q + ATT_STAGES * ATT_SMEM_STAGE +
-                                               ATT_SMEM_P);
-        // ---- sweep 1: row maximum ----
-        float mx = -3.0e38f;
-        for (int g = 0; g < nkb; ++g) {
-            const int slot = g % ATT_SLOTS;
-            mbar_wait(smem_u32(&s_full[slot]), (uint32_t)(g / ATT_SLOTS) & 1u);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = sub; c < ATT_BKEY / 32; c += 2) {
-                uint32_t v[32];
-                tmem_ld_32x32(t_row + 128u + (uint32_t)(slot * ATT_BKEY + c * 32), v);
-                tmem_ld_wait();
-                const int key0 = g * ATT_BKEY + c * 32;
-                if (key0 + 32 <= p.L) {
-#pragma unroll
-                    for (int t = 0; t < 32; ++t) mx = fmaxf(mx, __uint_as_float(v[t]));
-                } else {
-#pragma unroll
-                    for (int t = 0; t < 32; ++t)
-                        if (key0 + t < p.L) mx = fmaxf(mx, __uint_as_float(v[t]));
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(smem_u32(&s_empty[slot]));
-        }
-        xchg[sub * 128 + r] = mx;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        mx = fmaxf(mx, xchg[(sub ^ 1) * 128 + r]);
-        const float mscaled = mx * p.scale_log2e;
-        // ---- sweep 2: P_j and the row sum ----
-        float lsum = 0.f;
-        for (int j = 0; j < nkb; ++j) {
-            const int g = nkb + j, slot = g % ATT_SLOTS;
-            mbar_wait(smem_u32(&s_full[slot]), (uint32_t)(g / ATT_SLOTS) & 1u);
-            if (j > 0) mbar_wait(smem_u32(&p_empty), (uint32_t)(j - 1) & 1u);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = sub; c < ATT_BKEY / 32; c += 2) {
-                uint32_t v[32];
-                tmem_ld_32x32(t_row + 128u + (uint32_t)(slot * ATT_BKEY + c * 32), v);
-                tmem_ld_wait();
-                const int key0 = j * ATT_BKEY + c * 32;
-                const bool full = key0 + 32 <= p.L;
-                uint32_t hi[16], lo[16];
-#pragma unroll
-                for (int t = 0; t < 32; t += 2) {
-                    float e0, e1;
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(__uint_as_float(v[t]), p.scale_log2e, -mscaled)));
-                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(__uint_as_float(v[t + 1]), p.scale_log2e, -mscaled)));
-                    if (!full) {
-                        if (key0 + t >= p.L) e0 = 0.f;
-                        if (key0 + t + 1 >= p.L) e1 = 0.f;
-                    }
-                    lsum += e0 + e1;
-                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(e0, e1);
-                    const float2 hf = __bfloat1622float2(h2);
-                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(e0 - hf.x, e1 - hf.y);
-                    hi[t >> 1] = *reinterpret_cast<const uint32_t*>(&h2);
-                    lo[t >> 1] = *reinterpret_cast<const uint32_t*>(&l2);
-                }
-                const uint32_t rowbase = (uint32_t)((c >> 1) * ATT_TILE + r * 128);
-#pragma unroll
-                for (int q4 = 0; q4 < 4; ++q4) {
-                    const uint32_t chunk = (uint32_t)(((c & 1) * 4 + q4) ^ (r & 7));
-                    st_shared_v4(sP + rowbase + chunk * 16, hi[q4 * 4], hi[q4 * 4 + 1], hi[q4 * 4 + 2], hi[q4 * 4 + 3]);
-                    st_shared_v4(sP + 2 * ATT_TILE + rowbase + chunk * 16, lo[q4 * 4], lo[q4 * 4 + 1], lo[q4 * 4 + 2], lo[q4 * 4 + 3]);
-                }
-            }
-            tc_fence_before();
-            fence_proxy_async();
-            mbar_arrive(smem_u32(&s_empty[slot]));
-            mbar_arrive(smem_u32(&p_full));
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        xchg[sub * 128 + r] = lsum;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        lsum += xchg[(sub ^ 1) * 128 + r];
-        mbar_wait(smem_u32(&o_full), 0);
-        tc_fence_after();
-        const int qrow = q_tile * ATT_BQ + r;
-        const float inv = 1.0f / lsum;
-        __nv_bfloat16* ohi = p.out_hi + (long long)b * p.out_b + (long long)h * p.out_h + (long long)qrow * p.ldo;
-        __nv_bfloat16* olo = ohi + p.out_plane;
-        {
-            const int c = sub;
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)(c * 32), v);
-            tmem_ld_wait();
-            if (qrow < p.L) {
-#pragma unroll
-                for (int t = 0; t < 32; t += 8) {
-                    uint32_t hh[4], ll[4];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        __nv_bfloat16 h0, l0, h1, l1;
-                        split_bf16(__uint_as_float(v[t + 2 * u]) * inv, h0, l0);
-                        split_bf16(__uint_as_float(v[t + 2 * u + 1]) * inv, h1, l1);
-                        hh[u] = pack_bf16x2(h0, h1);
-                        ll[u] = pack_bf16x2(l0, l1);
-                    }
-                    *reinterpret_cast<uint4*>(ohi + c * 32 + t) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-                    *reinterpret_cast<uint4*>(olo + c * 32 + t) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-                }
-            }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-
-// ---------------------------------------------------------------------------------------------------------
-// attention_pair_kernel: the production path for dh = 64 at ANY sequence length.
-//
-// What bounds fused attention on this part (profiles/r02_attention_*): tensor memory is READ at only ~64 B/clk per SM, so
-// fetching a 128 x 128 fp32 S block costs as much (1024 clk) as exponentiating it on the MUFU pipe (1024 clk) and more than
-// the MMAs that produced it (768 clk, three split-bf16 passes); a kernel that fetches, then exponentiates, then stores with
-// one query tile per CTA leaves the tensor pipe idle for two thirds of the CTA's life (31 % active, round-2 streaming
-// kernel; 23 % round-1 two-pass kernel).  This kernel keeps every unit busy at once:
-//   * ONE CTA = TWO query tiles (256 queries) of one (cloud, head): K_j / V_j are loaded once for both tiles and the MMA
-//     warp alternates between them - items g = 2 j + t: S_g = Q_t K_j^T into TMEM slot g % 3, O_t += P_g V_j.  While softmax
-//     group t works on item g, the tensor pipe computes S_{g+1..g+2} and PV_{g-1} of the OTHER tile.
-//   * softmax group t = 4 warps, ONE THREAD PER QUERY ROW (all 128 keys of the block): no cross-thread exchange, no named
-//     barrier.  The row is processed in four 32-key chunks; tcgen05.ld of chunk k+1 is in flight while chunk k is
-//     exponentiated (FFMA2 / MUFU.EX2 / packed cvt) and written BACK IN PLACE as split-bf16 (hi in columns [32k, 32k+16),
-//     lo in [32k+16, 32k+32) of the slot, two keys per 32-bit column).  O_t += P_g V_j takes P as the TMEM A operand of
-//     tcgen05.mma and V^T as an MN-major shared-memory B operand (no transpose, no shared-memory round trip for P).
-//   * single pass with a LAZY reference maximum: P = exp2(S c - m_ref c).  softmax is shift invariant and every operand is
-//     floating point, so m_ref only has to keep P inside the exponent range: it is moved when a chunk maximum exceeds it by
-//     more than 2^AP_TAU (always at the first chunk of a row, practically never afterwards); the owning thread then rescales
-//     its row of O_t (tcgen05.ld -> mul -> tcgen05.st, after PV of the previous block has retired), its running sum and
-//     the chunks of the current block it has already written.
-// Exactness: the result equals softmax(QK^T c) V up to fp32 rounding (same split-bf16 operands as the other kernels).
-// ---------------------------------------------------------------------------------------------------------
-constexpr int AP_STAGES = 4;        // K / V blocks in flight (32 KB each)
-constexpr int AP_SLOTS = 2;         // S / P slots of 128 TMEM columns (with two query tiles: one per softmax group)
-constexpr float AP_TAU = 40.0f;     // log2 units
-constexpr int AP_THREADS = 352;     // warps 0-3: softmax group 0, 4-7: group 1, 8: TMA, 9: S issuer (+ TMEM allocation), 10: PV issuer
-constexpr int AP_SMEM_TOTAL = 2 * ATT_SMEM_Q + AP_STAGES * ATT_SMEM_STAGE + 1024;  // dh = 64: 2 Q tiles + 4 stages; dh = 88: 1 Q tile of 2 chunks + 2 stages of 2 chunks
-
-// D[tmem] (+)= A[tmem] * B[smem desc]: P is read from tensor memory (row = lane, two bf16 per 32-bit column along K)
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
-}
-
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)),
-        "l"(*reinterpret_cast<unsigned long long*>(&b)), "l"(*reinterpret_cast<unsigned long long*>(&c)));
-    return *reinterpret_cast<float2*>(&d);
-}
-
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)),
-        "l"(*reinterpret_cast<unsigned long long*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
-
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b) {
-    unsigned long long d;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(*reinterpret_cast<unsigned long long*>(&a)),
-        "l"(*reinterpret_cast<unsigned long long*>(&b)));
-    return *reinterpret_cast<float2*>(&d);
-}
 
 __device__ __forceinline__ float ex2f(float x) {
     float e;
@@ -633,320 +51,222 @@ __device__ __forceinline__ float ex2f(float x) {
     return e;
 }
 
-__device__ __forceinline__ float bf16lo_f(uint32_t packed) { return __uint_as_float(packed << 16); }
-__device__ __forceinline__ float bf16hi_f(uint32_t packed) { return __uint_as_float(packed & 0xffff0000u); }
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
 
-// DH = 64: one 64-column chunk per Q / K / V tile, two query tiles per CTA.
-// DH = 88 (EVA-giant): two 64-column chunks, the second holds columns 64..87 and zeros (TMA fills what lies beyond the head's
-// extent); S uses 4 + 2 k-steps, the PV operand [V_hi0 | V_lo0 | V_hi1 | V_lo1] is 256 wide (four 64-column N atoms 16 KB
-// apart), O_t takes 256 TMEM columns, so a CTA holds ONE query tile and the stage ring two blocks.
-template <int DH>
-__global__ void __launch_bounds__(AP_THREADS, 1)
-attention_pair_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                      const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
-    constexpr int NCH = DH <= 64 ? 1 : 2;                 // 64-column chunks of a head
-    constexpr int KS_LAST = DH <= 64 ? 4 : (DH - 64 + 15) / 16;  // 16-wide k-steps of the last chunk that hold data
-    constexpr int Q_BYTES = NCH * ATT_SMEM_Q;             // one query tile (all chunks, hi + lo)
-    constexpr int ST_BYTES = NCH * ATT_SMEM_STAGE;        // one K or V block
-    constexpr int STAGES = DH <= 64 ? AP_STAGES : 2;
-    constexpr int NT_MAX = DH <= 64 ? 2 : 1;              // query tiles per CTA
-    constexpr int OC = 128 * NCH;                         // TMEM columns of one O_t: [P V_hi | P V_lo] per chunk
+__device__ __forceinline__ uint32_t bf16x2_bits(float lo, float hi) {
+    const __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t*>(&h2);
+}
+
+// S = Q K^T for this warpgroup's 64 rows and one 64-key block: NCH chunks x {Q_hi K_hi, Q_lo K_hi, Q_hi K_lo}.
+template <int NCH, int KS_LAST>
+__device__ __forceinline__ void att_scores(float (&s)[32], uint32_t sq, uint32_t sk) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) s[i] = 0.f;
+    fence_acc(s);
+    wgmma_fence();
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) {
+            const uint64_t qd = gmma_desc_k(sq + ch * 2 * ATT_Q_TILE + (pass == 1 ? ATT_Q_TILE : 0));
+            const uint64_t kd = gmma_desc_k(sk + ch * 2 * ATT_KV_TILE + (pass == 2 ? ATT_KV_TILE : 0));
+#pragma unroll
+            for (int k = 0; k < (ch == NCH - 1 ? KS_LAST : 4); ++k) wgmma_ss<64>(s, qd + 2 * k, kd + 2 * k, 1u);
+        }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(s);
+}
+
+// Keys at or beyond L take no part: their scores become -inf.  Register i of the fragment holds key 8 (i / 4) + 2 (lane % 4) + i % 2.
+__device__ __forceinline__ void att_mask(float (&s)[32], int key0, int L, int lane) {
+    if (key0 + ATT_BKEY <= L) return;
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+        if (key0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= L) s[i] = __int_as_float(0xff800000);
+}
+
+template <int DH, bool TWO_PASS>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
+attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                       const __grid_constant__ CUtensorMap tmap_v, const AttnParams p) {
+    constexpr int NCH = DH <= 64 ? 1 : 2;                         // 64-column chunks of a head
+    constexpr int KS_LAST = DH <= 64 ? 4 : (DH - 64 + 15) / 16;   // 16-wide k-steps of the last chunk that hold data
+    using S = AttSmem<NCH>;
     pdl_launch_dependents();
     extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t q_full, pv_done[2];
-    __shared__ __align__(8) uint64_t kv_full[AP_STAGES], kv_empty[AP_STAGES];
-    __shared__ __align__(8) uint64_t s_full[AP_SLOTS], p_full[AP_SLOTS], slot_free[AP_SLOTS];
-    __shared__ uint32_t tmem_base_smem;
+    __shared__ __align__(8) uint64_t q_full, kv_full[ATT_STAGES], kv_empty[ATT_STAGES];
 
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    const uint32_t sQ = smem_base;                    // Q tile t at sQ + t * ATT_SMEM_Q (hi plane, lo plane)
-    const uint32_t sKV = sQ + NT_MAX * Q_BYTES;
+    const uint32_t sQ = smem_base;      // chunk ch: hi plane at sQ + ch * 2 * ATT_Q_TILE, lo plane ATT_Q_TILE further
+    const uint32_t sKV = sQ + S::Q;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int h = blockIdx.y, b = blockIdx.z;
-    const int tpc = min(p.tiles_per_cta, NT_MAX);
-    const int q_tile0 = blockIdx.x * tpc;                                      // first of the (up to) two query tiles
-    const int nt = min(tpc, (p.L + ATT_BQ - 1) / ATT_BQ - q_tile0);            // query tiles of this CTA
+    const int q_tile = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const int nkb = (p.L + ATT_BKEY - 1) / ATT_BKEY;
-    const int G = nt * nkb;                                                    // items: g = j * nt + t
 
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmap_q);
         tma_prefetch_desc(&tmap_k);
         tma_prefetch_desc(&tmap_v);
         mbar_init(smem_u32(&q_full), 1);
-        mbar_init(smem_u32(&pv_done[0]), 1);
-        mbar_init(smem_u32(&pv_done[1]), 1);
-        for (int s = 0; s < STAGES; ++s) {
+        for (int s = 0; s < ATT_STAGES; ++s) {
             mbar_init(smem_u32(&kv_full[s]), 1);
-            mbar_init(smem_u32(&kv_empty[s]), 1);
-        }
-        for (int s = 0; s < AP_SLOTS; ++s) {
-            mbar_init(smem_u32(&s_full[s]), 1);
-            mbar_init(smem_u32(&p_full[s]), 128);  // the 128 threads of one softmax group
-            mbar_init(smem_u32(&slot_free[s]), 1);
+            mbar_init(smem_u32(&kv_empty[s]), 2);  // one arrival per consumer warpgroup
         }
         fence_mbar_init();
     }
-    if (warp == 9) tmem_alloc(smem_u32(&tmem_base_smem), 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    const uint32_t t_o = tmem_base;           // O_t: columns [OC t, OC t + OC): per 64-column chunk of the head P V_hi then P V_lo
-    const uint32_t t_s = tmem_base + 256u;    // slot s: columns [256 + 128 s, +128)
-    pdl_wait();
-    if (threadIdx.x == 0) att_trace(p, 0);  // trace layout: 0 start | 1 q_full seen | 2 + 8 g + {0 S issued, 1 PV issued, 2 s_full seen, 3 first chunk fetched, 4 exps done, 5 p_full arrive} | 200 end
+    pdl_wait();  // everything above is independent of the previous kernel; its outputs are read only below
 
-    // One thread issues a tcgen05.mma every ~120 clk at best, whatever its size (tools/mma_issue_probe.cu: 122 clk for
-    // N = 64 and N = 128 from one thread, half that from two), and an item needs 12 + 16 of them: a single issuing warp was
-    // the bottleneck of this kernel (softmax warps idle half of the time, profiles/r02).  So TWO warps issue: warp 9 the
-    // S_g = Q_t K_j^T products, warp 10 the O_t += P_g [V_hi | V_lo] products.  The only ordering between them - S_{g+2}
-    // overwrites the slot PV_g reads P from - goes through slot_free (tcgen05.commit of PV_g, one barrier per slot).
-    // The stage ring carries K_0 V_0 K_1 V_1 ...: K_j at position 2 j (S issuer), V_j at 2 j + 1 (PV issuer); a block is
-    // released after its last use (tile nt - 1).
+    // Order in which the stage ring carries the blocks (the consumers take them in exactly this order):
+    //   two-pass: K_0 .. K_{nkb-1}, then K_0 V_0 K_1 V_1 ...;   streaming: K_0 V_0 K_1 V_1 ...
+    const int n_items = (TWO_PASS ? 3 : 2) * nkb;
     if (warp == 8) {
         if (lane == 0) {
             const uint32_t qb = smem_u32(&q_full);
-            mbar_arrive_expect_tx(qb, (uint32_t)(nt * Q_BYTES));
-            for (int t = 0; t < nt; ++t)
-                for (int ch = 0; ch < NCH; ++ch)  // one 3-D box per 64-column chunk: 64 x 128 rows x {hi, lo}
-                    tma_load_5d(sQ + t * Q_BYTES + ch * ATT_SMEM_Q, &tmap_q, qb, 64 * ch, (q_tile0 + t) * ATT_BQ, 0, h, b);
-            for (int i = 0; i < 2 * nkb; ++i) {
-                const int s = i % STAGES;
-                mbar_wait(smem_u32(&kv_empty[s]), ((uint32_t)(i / STAGES) & 1u) ^ 1u);
+            mbar_arrive_expect_tx(qb, (uint32_t)S::Q);
+            for (int ch = 0; ch < NCH; ++ch)  // one 3-D box per 64-column chunk: 64 x 128 rows x {hi, lo}
+                tma_load_5d(sQ + ch * 2 * ATT_Q_TILE, &tmap_q, qb, 64 * ch, q_tile * ATT_BQ, 0, h, b);
+            for (int i = 0; i < n_items; ++i) {
+                const int s = i % ATT_STAGES;
+                mbar_wait(smem_u32(&kv_empty[s]), ((uint32_t)(i / ATT_STAGES) & 1u) ^ 1u);
                 const uint32_t fb = smem_u32(&kv_full[s]);
-                mbar_arrive_expect_tx(fb, ST_BYTES);
+                mbar_arrive_expect_tx(fb, (uint32_t)S::STAGE);
+                const int i2 = TWO_PASS ? i - nkb : i;  // position in the K V K V ... sequence (< 0: first sweep)
+                const bool is_v = i2 >= 0 && (i2 & 1);
+                const int blk = i2 < 0 ? i : (i2 >> 1);
                 for (int ch = 0; ch < NCH; ++ch)
-                    tma_load_5d(sKV + s * ST_BYTES + ch * ATT_SMEM_STAGE, (i & 1) ? &tmap_v : &tmap_k, fb, 64 * ch, (i >> 1) * ATT_BKEY, 0, h, b);
+                    tma_load_5d(sKV + s * S::STAGE + ch * 2 * ATT_KV_TILE, is_v ? &tmap_v : &tmap_k, fb, 64 * ch, blk * ATT_BKEY, 0, h, b);
             }
         }
-    } else if (warp == 9) {
-        // ===================== S issuer =====================
-        constexpr uint32_t idesc_s = umma_idesc_bf16(128, ATT_BKEY);
-        mbar_wait(smem_u32(&q_full), 0);
-        tc_fence_after();
-        if (lane == 0) att_trace(p, 1);
-        for (int g = 0; g < G; ++g) {
-            const int t = g % nt, j = g / nt, slot = g % AP_SLOTS;
-            const int i = 2 * j, ks = i % STAGES;
-            if (t == 0) mbar_wait(smem_u32(&kv_full[ks]), (uint32_t)(i / STAGES) & 1u);  // first use of K_j
-            // PV_{g-2} has read the slot S_g overwrites.  One barrier per SLOT: its next completion is PV_g, which cannot happen
-            // before S_g is issued, so this parity wait can never be lapped.  (Waiting on the per-tile pv_done here deadlocked
-            // when a CTA holds a single query tile: PV_{g-1} may retire while this warp still waits for K_g, the barrier is then
-            // two phases ahead and the parity test waits for a completion that needs S_g.)
-            if (g >= AP_SLOTS) mbar_wait(smem_u32(&slot_free[slot]), (uint32_t)(g / AP_SLOTS - 1) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t d_s = t_s + (uint32_t)(slot * ATT_BKEY);
-#pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {  // Q_hi K_hi, Q_lo K_hi, Q_hi K_lo
-#pragma unroll
-                    for (int ch = 0; ch < NCH; ++ch) {
-                        const uint32_t sq = sQ + t * Q_BYTES + ch * ATT_SMEM_Q, sk = sKV + ks * ST_BYTES + ch * ATT_SMEM_STAGE;
-                        const uint64_t qd = umma_desc_k_sw128(sq + (pass == 1 ? ATT_TILE : 0));
-                        const uint64_t kd = umma_desc_k_sw128(sk + (pass == 2 ? ATT_TILE : 0));
-#pragma unroll
-                        for (int k = 0; k < (ch == NCH - 1 ? KS_LAST : 4); ++k)
-                            umma_bf16(d_s, qd + 2 * k, kd + 2 * k, idesc_s, (pass > 0 || ch > 0 || k > 0) ? 1u : 0u);
-                    }
-                }
-                if (t == nt - 1) umma_commit(smem_u32(&kv_empty[ks]));  // last use of K_j
-                umma_commit(smem_u32(&s_full[slot]));
-                att_trace(p, 2 + 8 * g + 0);
-            }
-            __syncwarp();
-        }
-    } else if (warp == 10) {
-        // ===================== PV issuer =====================
-        constexpr uint32_t idesc_o = umma_idesc_bf16(128, OC) | (1u << 16);  // B = [V_hi | V_lo] per chunk, MN-major; A (P) from TMEM
-        for (int g = 0; g < G; ++g) {
-            const int t = g % nt, j = g / nt, slot = g % AP_SLOTS;
-            const int i = 2 * j + 1, vs = i % STAGES;
-            if (t == 0) mbar_wait(smem_u32(&kv_full[vs]), (uint32_t)(i / STAGES) & 1u);  // first use of V_j
-            mbar_wait(smem_u32(&p_full[slot]), (uint32_t)(g / AP_SLOTS) & 1u);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sv = sKV + vs * ST_BYTES;
-                const uint64_t v_hi = umma_desc_mn_sw128(sv);
-                const uint32_t a0 = t_s + (uint32_t)(slot * ATT_BKEY), d_o = t_o + (uint32_t)(t * OC);
-                // The tensor-memory A operand is read at ~64 B/clk: a 128 x 16 P step costs 64 clk whatever N is, so both P
-                // planes run against the 128-wide B operand [V_hi | V_lo] (the lo tile is the next 64-wide N atom of the MN-major
-                // descriptor, 16 KB further): two passes of N = 128 instead of three of N = 64 - a third fewer P reads and MMA
-                // instructions, and the P_lo V_lo term comes for free.  O_t[:, 0:64] += P V_hi, O_t[:, 64:128] += P V_lo, summed
-                // in the epilogue.  k-step kk = 16 keys: P hi in 8 TMEM columns at 32 (kk / 2) + 8 (kk % 2) of the slot, lo 16
-                // columns further; V: 16 rows = 2048 B further per step
-#pragma unroll
-                for (int kk = 0; kk < ATT_BKEY / 16; ++kk)
-                    umma_bf16_ts(d_o, a0 + (uint32_t)(32 * (kk >> 1) + 8 * (kk & 1)), v_hi + (uint64_t)(kk * (2048 >> 4)), idesc_o,
-                                 (j > 0 || kk > 0) ? 1u : 0u);
-#pragma unroll
-                for (int kk = 0; kk < ATT_BKEY / 16; ++kk)
-                    umma_bf16_ts(d_o, a0 + (uint32_t)(32 * (kk >> 1) + 8 * (kk & 1) + 16), v_hi + (uint64_t)(kk * (2048 >> 4)), idesc_o, 1u);
-                if (t == nt - 1) umma_commit(smem_u32(&kv_empty[vs]));  // last use of V_j
-                umma_commit(smem_u32(&pv_done[t]));
-                umma_commit(smem_u32(&slot_free[slot]));
-                att_trace(p, 2 + 8 * g + 1);
-            }
-            __syncwarp();
-        }
-    } else if ((warp >> 2) < nt) {
-        // ===================== softmax group t: one thread per query row =====================
-        const int t = warp >> 2;                  // query tile / group
-        const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-        const int r = quarter * 32 + lane;        // row inside the tile == TMEM lane
-        const uint32_t lane_off = (uint32_t)(quarter * 32) << 16;
-        const uint32_t t_orow = t_o + lane_off + (uint32_t)(t * OC);
-        const float c = p.scale_log2e;
-        const float2 c2 = make_float2(c, c);
-        float mref = __int_as_float(0xff800000);  // -inf: the first chunk of the row sets the reference
-        float2 lsum2 = make_float2(0.f, 0.f);
-        for (int j = 0; j < nkb; ++j) {
-            const int g = j * nt + t, slot = g % AP_SLOTS;
-            mbar_wait(smem_u32(&s_full[slot]), (uint32_t)(g / AP_SLOTS) & 1u);
-            tc_fence_after();
-            const uint32_t t_slot = t_s + lane_off + (uint32_t)(slot * ATT_BKEY);
-            bool waited_pv = false;  // pv_done[t] completes one phase per block; each thread observes phase j-1 exactly once in block j
-            uint32_t va[32], vb[32];
-            if ((threadIdx.x & 127) == 0) att_trace(p, 2 + 8 * g + 2);
-            tmem_ld_32x32(t_slot, va);
-            // one 32-key chunk: v holds S (fetched earlier), vn receives the next chunk while this one is exponentiated
-            auto chunk = [&](int k, uint32_t (&v)[32], uint32_t (&vn)[32]) {
-                tmem_ld_wait();
-#pragma unroll
-                for (int i2 = 0; i2 < 32; ++i2) asm volatile("" : "+r"(v[i2]));  // v is defined from here on, not earlier
-                if (k + 1 < ATT_BKEY / 32) tmem_ld_32x32(t_slot + (uint32_t)(32 * (k + 1)), vn);
-                const int key0 = j * ATT_BKEY + k * 32;
-                if (key0 + 32 > p.L) {  // ragged tail: keys beyond L do not take part
-#pragma unroll
-                    for (int i2 = 0; i2 < 32; ++i2)
-                        if (key0 + i2 >= p.L) v[i2] = 0xff800000u;  // -inf
-                }
-                float cm = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
-#pragma unroll
-                for (int i2 = 2; i2 < 32; i2 += 2) cm = fmax3(cm, __uint_as_float(v[i2]), __uint_as_float(v[i2 + 1]));
-                const bool need = (cm - mref) * c > AP_TAU;  // false for a fully masked chunk (cm = -inf)
-                if (__any_sync(0xffffffffu, need)) {
-                    // move the reference of the rows that need it; everything accumulated under the old one is rescaled
-                    const float f = need ? ex2f((mref - cm) * c) : 1.0f;  // first chunk of a row: mref = -inf -> f = 0
-                    tmem_st_wait();  // P chunks written above are re-read below
-                    if (j > 0) {
-                        if (!waited_pv) mbar_wait(smem_u32(&pv_done[t]), (uint32_t)(j - 1) & 1u);
-                        waited_pv = true;
-                        tc_fence_after();
-#pragma unroll 1
-                        for (int hh = 0; hh < OC / 32; ++hh) {
-                            uint32_t o[32];
-                            tmem_ld_32x32(t_orow + (uint32_t)(hh * 32), o);
-                            tmem_ld_wait();
-#pragma unroll
-                            for (int i2 = 0; i2 < 32; ++i2) o[i2] = __float_as_uint(__uint_as_float(o[i2]) * f);
-                            tmem_st_32x32(t_orow + (uint32_t)(hh * 32), o);
-                        }
-                    }
-#pragma unroll 1
-                    for (int kk = 0; kk < k; ++kk) {  // chunks of this block already written as P under the old reference
-                        uint32_t pk[32];
-                        tmem_ld_32x32(t_slot + (uint32_t)(32 * kk), pk);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i2 = 0; i2 < 16; ++i2) {
-                            const float e0 = (bf16lo_f(pk[i2]) + bf16lo_f(pk[16 + i2])) * f;
-                            const float e1 = (bf16hi_f(pk[i2]) + bf16hi_f(pk[16 + i2])) * f;
-                            uint32_t h2, l2;
-                            asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h2) : "f"(e1), "f"(e0));
-                            asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(l2) : "f"(e1 - bf16hi_f(h2)), "f"(e0 - bf16lo_f(h2)));
-                            pk[i2] = h2, pk[16 + i2] = l2;
-                        }
-                        tmem_st_32x32(t_slot + (uint32_t)(32 * kk), pk);
-                    }
-                    lsum2.x *= f, lsum2.y *= f;
-                    if (need) mref = cm;
-                    // (the tcgen05.wait::ld above also completed the prefetch of the next chunk: harmless)
-                }
-                const float2 nm2 = make_float2(-mref * c, -mref * c);
-                uint32_t hl[32];  // hi pairs in [0,16), lo pairs in [16,32)
-#pragma unroll
-                for (int i2 = 0; i2 < 32; i2 += 2) {
-                    const float2 x = ffma2(make_float2(__uint_as_float(v[i2]), __uint_as_float(v[i2 + 1])), c2, nm2);
-                    const float2 e = make_float2(ex2f(x.x), ex2f(x.y));
-                    lsum2 = fadd2(lsum2, e);
-                    uint32_t h2;
-                    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h2) : "f"(e.y), "f"(e.x));
-                    const float2 d = fsub2(e, make_float2(bf16lo_f(h2), bf16hi_f(h2)));
-                    uint32_t l2;
-                    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(l2) : "f"(d.y), "f"(d.x));
-                    hl[i2 >> 1] = h2;
-                    hl[16 + (i2 >> 1)] = l2;
-                }
-                tmem_st_32x32(t_slot + (uint32_t)(32 * k), hl);  // in place: the 32 columns this chunk's S came from
-            };
-            chunk(0, va, vb);
-            if ((threadIdx.x & 127) == 0) att_trace(p, 2 + 8 * g + 3);
-            chunk(1, vb, va);
-            chunk(2, va, vb);
-            chunk(3, vb, va);
-            if ((threadIdx.x & 127) == 0) att_trace(p, 2 + 8 * g + 4);
-            if (j > 0 && !waited_pv) mbar_wait(smem_u32(&pv_done[t]), (uint32_t)(j - 1) & 1u);
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(smem_u32(&p_full[slot]));
-            if ((threadIdx.x & 127) == 0) att_trace(p, 2 + 8 * g + 5);
-        }
-        // ---- epilogue: O_t / rowsum -> split-bf16 [B*L, H*dh] ----
-        const float lsum = lsum2.x + lsum2.y;
-        mbar_wait(smem_u32(&pv_done[t]), (uint32_t)(nkb - 1) & 1u);
-        tc_fence_after();
-        const int qrow = (q_tile0 + t) * ATT_BQ + r;
-        const float inv = 1.0f / lsum;
-        __nv_bfloat16* ohi = p.out_hi + (long long)b * p.out_b + (long long)h * p.out_h + (long long)qrow * p.ldo;
-        __nv_bfloat16* olo = ohi + p.out_plane;
-#pragma unroll 1
-        for (int hh = 0; hh < (DH + 31) / 32; ++hh) {  // 32 output columns at a time: chunk hh / 2 of the head, half hh % 2 of it
-            uint32_t o[32], o2[32];
-            const uint32_t cbase = (uint32_t)((hh >> 1) * 128 + (hh & 1) * 32);
-            tmem_ld_32x32(t_orow + cbase, o);         // P V_hi
-            tmem_ld_32x32(t_orow + cbase + 64u, o2);  // P V_lo
-            tmem_ld_wait();
-#pragma unroll
-            for (int i2 = 0; i2 < 32; ++i2) o[i2] = __float_as_uint(__uint_as_float(o[i2]) + __uint_as_float(o2[i2]));
-            if (qrow < p.L) {
-#pragma unroll
-                for (int i2 = 0; i2 < 32; i2 += 8) {
-                    if (hh * 32 + i2 < DH) {  // DH = 88: the last group of 32 holds 24 columns
-                        uint32_t oh[4], ol[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            __nv_bfloat16 h0, l0, h1, l1;
-                            split_bf16(__uint_as_float(o[i2 + 2 * u]) * inv, h0, l0);
-                            split_bf16(__uint_as_float(o[i2 + 2 * u + 1]) * inv, h1, l1);
-                            oh[u] = pack_bf16x2(h0, h1);
-                            ol[u] = pack_bf16x2(l0, l1);
-                        }
-                        *reinterpret_cast<uint4*>(ohi + hh * 32 + i2) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-                        *reinterpret_cast<uint4*>(olo + hh * 32 + i2) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-                    }
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x == 0) att_trace(p, 200);
-    if (warp == 9) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    // ===================== consumer warpgroup: 64 query rows =====================
+    const int wg = warp >> 2;
+    const bool leader = (warp & 3) == 0 && lane == 0;  // releases stages for the warpgroup
+    const uint32_t sq = sQ + wg * (ATT_Q_TILE / 2);
+    const float c = p.scale_log2e;
+    mbar_wait(smem_u32(&q_full), 0);
+    int item = 0;
+    auto acquire = [&]() {
+        const int s = item % ATT_STAGES;
+        mbar_wait(smem_u32(&kv_full[s]), (uint32_t)(item / ATT_STAGES) & 1u);
+        return sKV + s * S::STAGE;
+    };
+    auto release = [&]() {
+        if (leader) mbar_arrive(smem_u32(&kv_empty[item % ATT_STAGES]));
+        ++item;
+    };
+
+    float m[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};  // running maxima of the thread's two rows
+    float s[32];
+    if (TWO_PASS) {
+        for (int j = 0; j < nkb; ++j) {
+            att_scores<NCH, KS_LAST>(s, sq, acquire());
+            release();
+            att_mask(s, j * ATT_BKEY, p.L, lane);
+#pragma unroll
+            for (int i = 0; i < 32; ++i) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], s[i]);
+        }
+        m[0] = quad_max(m[0]);
+        m[1] = quad_max(m[1]);
+    }
+    float o[NCH][32];
+#pragma unroll
+    for (int ch = 0; ch < NCH; ++ch)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[ch][i] = 0.f;
+    float l[2] = {0.f, 0.f};  // partial row sums (this thread's columns)
+    for (int j = 0; j < nkb; ++j) {
+        att_scores<NCH, KS_LAST>(s, sq, acquire());
+        release();
+        att_mask(s, j * ATT_BKEY, p.L, lane);
+        if (!TWO_PASS) {
+            float mb[2] = {m[0], m[1]};
+#pragma unroll
+            for (int i = 0; i < 32; ++i) mb[(i >> 1) & 1] = fmaxf(mb[(i >> 1) & 1], s[i]);
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                mb[q] = quad_max(mb[q]);  // finite: every block holds at least one key < L
+                const float f = ex2f((m[q] - mb[q]) * c);  // first block: m = -inf -> f = 0
+                l[q] *= f;
+#pragma unroll
+                for (int ch = 0; ch < NCH; ++ch)
+#pragma unroll
+                    for (int i = 0; i < 32; ++i)
+                        if (((i >> 1) & 1) == q) o[ch][i] *= f;
+                m[q] = mb[q];
+            }
+        }
+        // P = exp2(S c - m c) split into bf16 hi / lo: k-step kk (16 keys) uses registers 8 kk .. 8 kk + 7
+        uint32_t ph[4][4], pl[4][4];
+        const float nm[2] = {-m[0] * c, -m[1] * c};
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int i = 8 * kk + 2 * r, q = r & 1;
+                const float e0 = ex2f(fmaf(s[i], c, nm[q])), e1 = ex2f(fmaf(s[i + 1], c, nm[q]));
+                l[q] += e0 + e1;
+                ph[kk][r] = bf16x2_bits(e0, e1);
+                const float2 hf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ph[kk][r]));
+                pl[kk][r] = bf16x2_bits(e0 - hf.x, e1 - hf.y);
+            }
+        }
+        const uint32_t sv = acquire();
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) fence_acc(o[ch]);
+        wgmma_fence();
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) {
+            const uint64_t v_hi = gmma_desc_mn64(sv + ch * 2 * ATT_KV_TILE), v_lo = gmma_desc_mn64(sv + ch * 2 * ATT_KV_TILE + ATT_KV_TILE);
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {  // V: 16 rows = 2048 B further per k-step
+                wgmma_rs_tb<64>(o[ch], ph[kk], v_hi + (uint64_t)(kk * (2048 >> 4)));
+                wgmma_rs_tb<64>(o[ch], pl[kk], v_hi + (uint64_t)(kk * (2048 >> 4)));
+                wgmma_rs_tb<64>(o[ch], ph[kk], v_lo + (uint64_t)(kk * (2048 >> 4)));
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) fence_acc(o[ch]);
+        release();
+    }
+    // ---- epilogue: O / rowsum -> split-bf16 [B*L, H*dh] ----
+    const int rbase = q_tile * ATT_BQ + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        float lq = l[q] + __shfl_xor_sync(0xffffffffu, l[q], 1);
+        lq += __shfl_xor_sync(0xffffffffu, lq, 2);
+        const float inv = 1.0f / lq;
+        const int row = rbase + 8 * q;
+        if (row >= p.L) continue;
+        __nv_bfloat16* ohi = p.out_hi + (long long)b * p.out_b + (long long)h * p.out_h + (long long)row * p.ldo;
+        __nv_bfloat16* olo = ohi + p.out_plane;
+#pragma unroll
+        for (int ch = 0; ch < NCH; ++ch) {
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+                const int col = ch * 64 + 8 * g + 2 * (lane & 3);
+                if (col >= DH) continue;
+                __nv_bfloat16 h0, l0, h1, l1;
+                split_bf16(o[ch][4 * g + 2 * q] * inv, h0, l0);
+                split_bf16(o[ch][4 * g + 2 * q + 1] * inv, h1, l1);
+                *reinterpret_cast<uint32_t*>(ohi + col) = pack_bf16x2(h0, h1);
+                *reinterpret_cast<uint32_t*>(olo + col) = pack_bf16x2(l0, l1);
+            }
+        }
     }
 }
 
 int make_operand_map_ext(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes);  // gemm_tc.cu
-
-}  // namespace psam
-
-namespace psam {
-
-static unsigned long long* g_attention_trace = nullptr;  // tools/attention_trace.py only (psam_debug_attention_trace)
-static int g_attention_tiles_per_cta = 2;                // experiment switch (psam_debug_attention_tiles): 1 or 2 query tiles per CTA
 
 static int attention_setup(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi, long long out_plane,
                            long long ldo, long long out_head_stride, long long out_cloud_stride, float scale, CUtensorMap* mq,
@@ -967,16 +287,22 @@ static int attention_setup(const psam_operand* q, const psam_operand* k, const p
     p->scale_log2e = scale * 1.4426950408889634f;
     p->out_hi = (__nv_bfloat16*)out_hi;
     p->out_plane = out_plane, p->ldo = ldo, p->out_h = out_head_stride, p->out_b = out_cloud_stride;
-    p->trace = g_attention_trace;
-    p->tiles_per_cta = g_attention_tiles_per_cta;
     *grid = dim3((unsigned)ceil_div(L, ATT_BQ), (unsigned)H, (unsigned)B);
     return PSAM_OK;
 }
 
-}  // namespace psam
+template <int DH, bool TWO_PASS>
+static int launch_attention(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttnParams& p, dim3 grid,
+                            cudaStream_t stream) {
+    auto kern = attention_wgmma_kernel<DH, TWO_PASS>;
+    constexpr int smem = AttSmem<DH <= 64 ? 1 : 2>::TOTAL;
+    PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    PSAM_CUDA_TRY(psam::launch(kern, grid, dim3(ATT_THREADS), (size_t)smem, stream, mq, mk, mv, p));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
 
-extern "C" void psam_debug_attention_trace(unsigned long long* device_buffer) { psam::g_attention_trace = device_buffer; }
-extern "C" void psam_debug_attention_tiles(int tiles_per_cta) { psam::g_attention_tiles_per_cta = tiles_per_cta == 1 ? 1 : 2; }
+}  // namespace psam
 
 extern "C" int psam_attention_bf16x3(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi,
                                      long long out_plane, long long ldo, long long out_head_stride,
@@ -987,17 +313,8 @@ extern "C" int psam_attention_bf16x3(const psam_operand* q, const psam_operand* 
     dim3 grid;
     int rc = attention_setup(q, k, v, out_hi, out_plane, ldo, out_head_stride, out_cloud_stride, scale, &mq, &mk, &mv, &p, &grid);
     if (rc) return rc;
-    if (q->k == 88) {  // EVA-giant heads: one query tile per CTA
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(attention_pair_kernel<88>, cudaFuncAttributeMaxDynamicSharedMemorySize, AP_SMEM_TOTAL));
-        PSAM_CUDA_TRY(psam::launch(attention_pair_kernel<88>, dim3(grid), dim3(AP_THREADS), (size_t)(AP_SMEM_TOTAL), stream, mq, mk, mv, p));
-        PSAM_LAUNCH_CHECK();
-        return PSAM_OK;
-    }
-    grid.x = (grid.x + p.tiles_per_cta - 1) / p.tiles_per_cta;  // one or two query tiles per CTA
-    PSAM_CUDA_TRY(cudaFuncSetAttribute(attention_pair_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, AP_SMEM_TOTAL));
-    PSAM_CUDA_TRY(psam::launch(attention_pair_kernel<64>, dim3(grid), dim3(AP_THREADS), (size_t)(AP_SMEM_TOTAL), stream, mq, mk, mv, p));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
+    if (q->k == 88) return launch_attention<88, false>(mq, mk, mv, p, grid, stream);
+    return launch_attention<64, false>(mq, mk, mv, p, grid, stream);
 }
 
 extern "C" int psam_attention_bf16x3_twopass(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi,
@@ -1007,17 +324,8 @@ extern "C" int psam_attention_bf16x3_twopass(const psam_operand* q, const psam_o
     CUtensorMap mq, mk, mv;
     AttnParams p;
     dim3 grid;
-    if (q && q->k != ATT_DH) return PSAM_ERR_UNSUPPORTED;  // the first-generation kernels cover dh = 64 only
+    if (q && q->k != 64) return PSAM_ERR_UNSUPPORTED;  // the two-pass form covers dh = 64 only
     int rc = attention_setup(q, k, v, out_hi, out_plane, ldo, out_head_stride, out_cloud_stride, scale, &mq, &mk, &mv, &p, &grid);
     if (rc) return rc;
-    if (p.L > 512) {  // two-sweep kernel: S streamed through a ring of TMEM slots
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(attention_tc_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_TOTAL));
-        attention_tc_long_kernel<<<grid, ATT_THREADS, ATT_SMEM_TOTAL, stream>>>(mq, mk, mv, p);
-        PSAM_LAUNCH_CHECK();
-        return PSAM_OK;
-    }
-    PSAM_CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_TOTAL));
-    PSAM_CUDA_TRY(psam::launch(attention_tc_kernel, dim3(grid), dim3(ATT_THREADS), (size_t)(ATT_SMEM_TOTAL), stream, mq, mk, mv, p));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
+    return launch_attention<64, true>(mq, mk, mv, p, grid, stream);
 }

@@ -925,7 +925,7 @@ __global__ void __launch_bounds__(256) linear_gemv_ksplit_kernel(const psam_line
     }
 }
 
-static inline int grid_for(long long work, int per_block, int max_blocks = 148 * 32) {
+static inline int grid_for(long long work, int per_block, int max_blocks = 132 * 32) {
     long long g = (work + per_block - 1) / per_block;
     if (g < 1) g = 1;
     if (g > max_blocks) g = max_blocks;
@@ -1008,7 +1008,7 @@ extern "C" int psam_small_in_linear(const float* x, int rows, int Cin, const flo
     if (!x || !W || !y_hi || rows <= 0 || Cin <= 0 || Cin > 16 || Cout % 32 || Cout <= 0 || Cout > 512) return PSAM_ERR_ARG;
     if (use_ln && (!gamma || !beta)) return PSAM_ERR_ARG;
     const size_t smem = (size_t)(Cout * Cin + Cout) * sizeof(float);
-    const int blocks = grid_for(rows, 8, 148 * 8);
+    const int blocks = grid_for(rows, 8, 132 * 8);
     __nv_bfloat16* yh = (__nv_bfloat16*)y_hi;
 #define PSAM_SIL(CPL)                                                                                                     \
     PSAM_CUDA_TRY(psam::launch(small_in_linear_kernel<CPL>, dim3(blocks), dim3(256), (size_t)(smem), stream, x, rows, Cin, W, b, gamma, beta, eps, use_ln, act, yh, \
@@ -1128,7 +1128,7 @@ extern "C" int psam_mask_dot(const float* u, long long ldu, const float* hyper, 
                              cudaStream_t stream) {
     if (!u || !hyper || !masks || Z <= 0 || C <= 0 || C > 8 || N <= 0 || D <= 0) return PSAM_ERR_ARG;
     const size_t smem = (size_t)C * D * sizeof(float);
-    dim3 grid(grid_for(N, 8, 148 * 8), Z);
+    dim3 grid(grid_for(N, 8, 132 * 8), Z);
     PSAM_CUDA_TRY(psam::launch(mask_dot_kernel, dim3(grid), dim3(256), (size_t)(smem), stream, u, ldu, hyper, Z, C, N, D, masks));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
@@ -1188,7 +1188,7 @@ extern "C" int psam_linear_f32(const psam_linear_args* a, cudaStream_t stream) {
     return PSAM_OK;
 }
 
-extern "C" const char* psam_version(void) { return "psam_b200 0.1 (sm_100a)"; }
+extern "C" const char* psam_version(void) { return "psam_b200 0.1 (sm_90a)"; }
 
 extern "C" int psam_voronoi_features_f32(const float* xyz, const float* centers, const long long* nn_idx, const float* feats, int B,
                                          int rep, int N, int G, int C, float* out, void* y_hi, long long y_plane, long long pitch,
@@ -1197,7 +1197,7 @@ extern "C" int psam_voronoi_features_f32(const float* xyz, const float* centers,
     if (!xyz || !centers || !nn_idx || !feats || (!out && !y_hi) || B <= 0 || rep <= 0 || N <= 0 || G <= 0 || C < 0) return PSAM_ERR_ARG;
     if (y_hi && pitch < 4 + C) return PSAM_ERR_ARG;
     const long long total = (long long)B * rep * N;
-    const int blocks = (int)min((long long)148 * 16, ceil_div_ll(total, 256));
+    const int blocks = (int)min((long long)132 * 16, ceil_div_ll(total, 256));
     PSAM_CUDA_TRY(psam::launch(voronoi_features_kernel, dim3(blocks), dim3(256), (size_t)0, stream, xyz, centers, nn_idx, feats, B * rep, rep, N, G,
                                C, out, (__nv_bfloat16*)y_hi, y_plane, pitch));
     PSAM_LAUNCH_CHECK();
@@ -1211,10 +1211,10 @@ extern "C" int psam_scatter_amax_f32(const float* x, const long long* nn_idx, in
     const long long n = (long long)B * G * D;
     {
         // -inf fill, scatter, reset of the empty cells
-        const int fb = (int)min((long long)148 * 8, ceil_div_ll(n, 256));
+        const int fb = (int)min((long long)132 * 8, ceil_div_ll(n, 256));
         PSAM_CUDA_TRY(psam::launch(fill_f32_kernel, dim3(fb), dim3(256), (size_t)0, stream, y, n, -INFINITY));
         const long long work = (long long)B * N * (D / 4);
-        const int sb = (int)min((long long)148 * 16, ceil_div_ll(work, 256));
+        const int sb = (int)min((long long)132 * 16, ceil_div_ll(work, 256));
         PSAM_CUDA_TRY(psam::launch(scatter_amax_kernel, dim3(sb), dim3(256), (size_t)0, stream, x, nn_idx, (long long)B * N, N, G, D, y));
         PSAM_CUDA_TRY(psam::launch(scatter_amax_finish_kernel, dim3(fb), dim3(256), (size_t)0, stream, y, n));
     }

@@ -1,4 +1,4 @@
-// Farthest-point sampling for sm_100a.
+// Farthest-point sampling for sm_90a.
 //
 // Replaces torkit3d's sample_farthest_points_cuda
 // (third_party/torkit3d/torkit3d/csrc/cuda/sample_farthest_points_kernel.cu:8-165) and the
@@ -16,7 +16,7 @@
 //
 // Bit-exactness: squared distance is fmaf(dz,dz,fmaf(dy,dy,dx*dx)) with d = p_j - p_sel, and among
 // equal maxima the winner is the lexicographic minimum of (bitrev(j mod T), j div T), T = the
-// reference's block size for this N (SURVEY.md section 8 a-1); if the maximum is 0 the previous index
+// reference's block size for this N; if the maximum is 0 the previous index
 // is repeated.  Independent of how points are distributed over threads here.
 #include "psam_common.cuh"
 #include "../../include/psam_b200.h"

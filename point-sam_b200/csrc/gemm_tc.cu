@@ -1,26 +1,25 @@
-// Tensor-core GEMM for sm_100a: C[M,N] = A[M,K] * W[N,K]^T (+bias, activation, residual).
+// Tensor-core GEMM for sm_90a: C[M,N] = A[M,K] * W[N,K]^T (+bias, activation, residual).
 //
 // Replaces every nn.Linear / bmm of the reference hot path that has enough rows to fill a 128-row
 // MMA tile (PatchEncoder common.py:486-497, patch_proj/pos_embed/out_proj pc_encoder.py:99-116, the
 // timm EVA block linears and attention products, output_upscaling mask_decoder.py:53-59).
 //
 // Numerics ("split-bf16"): the reference runs these contractions in fp32.  Operands are stored as two
-// bf16 planes, x = hi + lo (relative residual <= 2^-17), and the product is accumulated in fp32 TMEM as
+// bf16 planes, x = hi + lo (relative residual <= 2^-17), and the product is accumulated in fp32 registers as
 //        A_hi*W_hi + A_lo*W_hi + A_hi*W_lo                                   (passes = 3)
-// which keeps ~16 mantissa bits per operand: measured end-to-end logit error ~2e-5 vs fp32, inside the
+// which keeps ~16 mantissa bits per operand: end-to-end logit error ~2e-5 vs fp32, inside the
 // 1e-3 abs / 1e-2 rel parity bound (a single bf16 pass, passes = 1, is ~1e-2 and fails it).
 //
 // Structure (one 128 x BN output tile per CTA, optional split-K over blockIdx.z):
-//   warp 0   : TMA producer (two lanes: A and W) - 5-D tensor maps (k, row, plane, batch1, batch2),
-//              128B-swizzled 3-D boxes of 64 bf16 x {128|BN} rows x {hi,lo}, 2-4 stage mbarrier ring
-//   warp 1   : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128xBNx16, kind::f16),
-//              tcgen05.commit releases smem stages and finally signals the epilogue
-//   warps 2-9: epilogue - tcgen05.ld 32x32b (warp owns TMEM lane quarter warp_id % 4; two warps per quarter
-//              split the column chunks), per-warp
-//              shared-memory transpose so that every global access is a contiguous row segment,
+//   warp 8   : TMA producer - 5-D tensor maps (k, row, plane, batch1, batch2), 128B-swizzled 3-D boxes of
+//              64 bf16 x {128|BN} rows x {hi,lo}, 2-4 stage mbarrier ring
+//   warps 0-7: two consumer warpgroups (rows 0-63 / 64-127 of the tile), wgmma m64nBNk16 from shared memory
+//              into fp32 registers; one wgmma group stays in flight while the previous stage is released.
+//              Epilogue: the accumulators are staged as an fp32 tile in the (then idle) stage memory, and each
+//              warp takes 32-row x 32-column chunks of it, so every global access is a contiguous row segment:
 //              bias/activation/residual, fp32 and/or split-bf16 stores (red.add for split-K)
-// The output-tile width BN is a runtime multiple of 32 (UMMA N and the TMA box follow it) chosen so the
-// tile count fits the 148 SMs in as few waves as possible.
+// The output-tile width BN is 64, 128 or 256 (the wgmma N), chosen so the tile count fills the 132 SMs of an
+// H100 in as few waves as possible.
 #include <stdlib.h>
 
 #include <cstdlib>
@@ -31,12 +30,11 @@ namespace psam {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_EPI_PER_QUARTER = 4;                         // default: 16 epilogue warps (four per TMEM lane quarter)
-constexpr int gemm_threads(int epq) { return 64 + 128 * epq; }  // TMA warp, MMA warp, 4*epq epilogue warps
-constexpr int GEMM_THREADS = gemm_threads(GEMM_EPI_PER_QUARTER);
-// psam_gemm_out.variant bits (experiment / policy switches; no environment variable is read inside the library)
-constexpr int GV_2CTA = 0x1, GV_BK32 = 0x2, GV_SCALAR_EPI = 0x4, GV_DUAL = 0x8, GV_NO_DUAL = 0x10, GV_PERSIST = 0x20, GV_NO_PERSIST = 0x40,
-              GV_TWO_ISSUERS = 0x80;
+constexpr int GEMM_THREADS = 288;  // two consumer warpgroups + one TMA warp
+constexpr int GEMM_A_TILE = GEMM_BM * GEMM_BK * 2;  // bytes per plane of an A stage
+// psam_gemm_out.variant bits.  GV_SCALAR_EPI forces the scalar epilogue; the other bits select kernels of other
+// architectures and are accepted without effect, so callers built for them keep working.
+constexpr int GV_SCALAR_EPI = 0x4;
 
 struct GemmEpilogue {
     float* out_f32;            // may be null
@@ -68,32 +66,30 @@ struct GemmShape {
     int nb1, nb2;  // batch extents (blockIdx.z = ((b2 * nb1) + b1) * split_k + split)
     int split_k;
     int passes;  // 1 or 3
-    int bn;      // output-tile width actually used (multiple of 32, <= MAXBN)
-    int cm;      // cluster size along M (1, 2 or 4): the CTAs of a cluster share the W tile through TMA multicast
-    int prefetch;  // k-blocks of W to prefetch into L2 ahead of the TMA loads (0 = off)
+    int bn;      // output-tile width (64, 128 or 256)
 };
 
-template <int MAXBN, int STAGES, int BK = 64>
+template <int BN, int STAGES>
 struct GemmSmem {
-    static constexpr int A_TILE = GEMM_BM * BK * 2;  // bytes per plane
-    static constexpr int B_TILE = MAXBN * BK * 2;
-    static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
-    static constexpr int TOTAL = STAGES * STAGE + 1024;  // + alignment slack
-    static constexpr int TMEM_COLS = MAXBN <= 64 ? 64 : (MAXBN <= 128 ? 128 : 256);
+    static constexpr int B_TILE = BN * GEMM_BK * 2;  // bytes per plane
+    static constexpr int STAGE = 2 * GEMM_A_TILE + 2 * B_TILE;
+    static constexpr int PITCH = BN + 4;              // floats per row of the staged output tile
+    static constexpr int EPI = GEMM_BM * PITCH * 4;   // the staged tile reuses the stage memory
+    static constexpr int TOTAL = (STAGES * STAGE > EPI ? STAGES * STAGE : EPI) + 1024;  // + alignment slack
+    static_assert(TOTAL <= 232448, "shared memory of one H100 SM");
 };
-
 
 // ---- epilogue row loops, specialised at compile time (runtime flags inside the loop cost ~10 uniform
 //      branches per row and made the epilogue the slowest part of small-K GEMMs) -------------------------
 template <int ACT, bool RES, bool ACC>
-__device__ __forceinline__ void epi_rows_f32(const float* __restrict__ stg, int lane, int row0, int M, int col, bool col_ok,
-                                             float alpha, float bv, float* out, const float* res, long long ldo) {
+__device__ __forceinline__ void epi_rows_f32(const float* __restrict__ stg, int pitch, int lane, int row0, int M, int col,
+                                             bool col_ok, float alpha, float bv, float* out, const float* res, long long ldo) {
     if (!col_ok) return;
 #pragma unroll 8
     for (int r = 0; r < 32; ++r) {
         const int row = row0 + r;
         if (row < M) {
-            float x = fmaf(stg[r * 33 + lane], alpha, bv);
+            float x = fmaf(stg[r * pitch + lane], alpha, bv);
             if (RES) x += res[(long long)row * ldo + col];
             x = apply_act(x, ACT);
             if (ACC) atomicAdd(out + (long long)row * ldo + col, x);
@@ -106,19 +102,19 @@ __device__ __forceinline__ void epi_rows_f32(const float* __restrict__ stg, int 
 // SwiGLU epilogue: W rows are interleaved (2i = gate_i, 2i+1 = value_i) so adjacent lanes hold a pair;
 // out[row, col/2] = silu(acc_g + b_g) * (acc_x + b_x).  Halves the fc1 output traffic and removes the
 // activation from the LayerNorm kernel that follows (timm SwiGLU: x = act(fc1_g(x)) * fc1_x(x)).
-__device__ __forceinline__ void epi_rows_swiglu(const float* __restrict__ stg, int lane, int row0, int M, int col, bool col_ok,
-                                                float alpha, float bv, float* out, long long ldo) {
+__device__ __forceinline__ void epi_rows_swiglu(const float* __restrict__ stg, int pitch, int lane, int row0, int M, int col,
+                                                bool col_ok, float alpha, float bv, float* out, long long ldo) {
 #pragma unroll 8
     for (int r = 0; r < 32; ++r) {
         const int row = row0 + r;
-        const float x = fmaf(stg[r * 33 + lane], alpha, bv);
+        const float x = fmaf(stg[r * pitch + lane], alpha, bv);
         const float other = __shfl_xor_sync(0xffffffffu, x, 1);
         if (row < M && col_ok && (lane & 1) == 0) out[(long long)row * ldo + (col >> 1)] = __fdividef(x, 1.0f + __expf(-x)) * other;
     }
 }
 
 template <int ACT, bool RES, bool F32>
-__device__ __forceinline__ void epi_rows_split(const float* __restrict__ stg, int lane, int row0, int M, int N, int col0,
+__device__ __forceinline__ void epi_rows_split(const float* __restrict__ stg, int pitch, int lane, int row0, int M, int N, int col0,
                                                float alpha, const float* bias, float* out, const float* res, long long ldo,
                                                __nv_bfloat16* ohi, long long out_plane, long long ldo_s, bool vec_align) {
     // lanes 0..15 take row r, lanes 16..31 row r+1, two adjacent columns each
@@ -133,8 +129,8 @@ __device__ __forceinline__ void epi_rows_split(const float* __restrict__ stg, in
     for (int r = 0; r < 32; r += 2) {
         const int row = row0 + r + half;
         if (row < M) {
-            float x0 = fmaf(stg[(r + half) * 33 + cpair], alpha, bv0);
-            float x1 = fmaf(stg[(r + half) * 33 + cpair + 1], alpha, bv1);
+            float x0 = fmaf(stg[(r + half) * pitch + cpair], alpha, bv0);
+            float x1 = fmaf(stg[(r + half) * pitch + cpair + 1], alpha, bv1);
             if (RES) {
                 if (ok0) x0 += res[(long long)row * ldo + c0];
                 if (ok1) x1 += res[(long long)row * ldo + c0 + 1];
@@ -161,46 +157,23 @@ __device__ __forceinline__ void epi_rows_split(const float* __restrict__ stg, in
 }
 
 
-// K-major shared-memory matrix descriptor for a tile whose rows hold BK bf16: BK=64 -> 128-byte rows / SWIZZLE_128B
-// (8-row groups 1024 B apart), BK=32 -> 64-byte rows / SWIZZLE_64B (8-row groups 512 B apart).
-template <int BK>
-__device__ __forceinline__ uint64_t umma_desc_k(uint32_t smem_addr) {
-    if (BK == 64) return umma_desc_k_sw128(smem_addr);
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(512 >> 4) << 32;  // stride byte offset between 8-row groups
-    d |= (uint64_t)1 << 46;           // descriptor version (sm_100)
-    d |= (uint64_t)4 << 61;           // layout type SWIZZLE_64B
-    return d;
-}
-
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {
     if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
 // ---- vectorised epilogue (fast path) -------------------------------------------------------------------------------
-// One 32-row x 32-column chunk per call.  Staging is a 128-bit transpose through shared memory: thread = row writes its 32
-// accumulators as 8 STS.128 (row pitch 36 floats: conflict-free), then lane (rsub = lane/8, cg = lane%8) reads rows
-// rsub, rsub+4, ... as float4 at columns 4*cg..4*cg+3, so every global instruction of the warp covers 4 rows x 128
-// contiguous bytes.  8 LDS.128 + 8 STG.128 (or 16 STG.64 for the split planes) per chunk instead of 32 + 32 scalar ones:
-// the scalar epilogue issued ~0.9 warp-instructions per output element and bounded the small-K GEMMs of the mini-PointNet.
-constexpr int EPI_PITCH = 36;  // floats per staged row
+// One 32-row x 32-column chunk of the staged fp32 tile per call: lane (rsub = lane/8, cg = lane%8) reads rows rsub,
+// rsub+4, ... as float4 at columns 4*cg..4*cg+3, so every global instruction of the warp covers 4 rows x 128 contiguous
+// bytes (8 LDS.128 + 8 STG.128, or 16 STG.64 for the split planes, per chunk instead of 32 + 32 scalar ones).
 enum EpiMode { EPI_F32 = 0, EPI_ACC = 1, EPI_SPLIT = 2, EPI_SPLIT_F32 = 3, EPI_SWIGLU = 4, EPI_NONE = 5, EPI_SWIGLU_SPLIT = 6 };
 
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 
 template <int ACT, bool RES, int MODE>
-__device__ __forceinline__ void epi_chunk_v4(float* __restrict__ stg, const uint32_t (&v)[32], int lane, int row0, int M, int col0,
+__device__ __forceinline__ void epi_chunk_v4(const float* __restrict__ stg, int pitch, int lane, int row0, int M, int col0,
                                              const GemmEpilogue& ep, bool add_bias, float* out, const float* res,
                                              __nv_bfloat16* ohi) {
-    float4* srow = reinterpret_cast<float4*>(stg + lane * EPI_PITCH);
-    __syncwarp();
-#pragma unroll
-    for (int q = 0; q < 8; ++q)
-        srow[q] = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                              __uint_as_float(v[4 * q + 3]));
-    __syncwarp();
     const int cg = lane & 7, rsub = lane >> 3;
     const int col = col0 + cg * 4;
     const float4 b4 = add_bias ? ld4(ep.bias + col) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -213,7 +186,7 @@ __device__ __forceinline__ void epi_chunk_v4(float* __restrict__ stg, const uint
     for (int i = 0; i < 8; ++i) {
         const int rr = i * 4 + rsub, row = row0 + rr;
         const bool ok = row < M;
-        float4 x = ld4(stg + rr * EPI_PITCH + cg * 4);
+        float4 x = ld4(stg + rr * pitch + cg * 4);
         // pre-activation: plain alpha*acc + bias, or the LayerNorm folded into this GEMM (A = un-normalised rows, W scaled by
         // gamma): rstd * (acc - mean * c[n]) + bias'[n] with the row statistics accumulated by the producer of A
         if (ep.ln_stats) {
@@ -307,10 +280,10 @@ __device__ __forceinline__ void epi_chunk_v4(float* __restrict__ stg, const uint
 }
 
 template <int ACT>
-__device__ __forceinline__ void epi_chunk_v4_dispatch(float* stg, const uint32_t (&v)[32], int lane, int row0, int M, int col0,
+__device__ __forceinline__ void epi_chunk_v4_dispatch(const float* stg, int pitch, int lane, int row0, int M, int col0,
                                                       const GemmEpilogue& ep, bool add_bias, float* out, const float* res,
                                                       __nv_bfloat16* ohi) {
-#define PSAM_V4(R, MODE) epi_chunk_v4<ACT, R, MODE>(stg, v, lane, row0, M, col0, ep, add_bias, out, res, ohi)
+#define PSAM_V4(R, MODE) epi_chunk_v4<ACT, R, MODE>(stg, pitch, lane, row0, M, col0, ep, add_bias, out, res, ohi)
     if (ep.swiglu && ohi) PSAM_V4(false, EPI_SWIGLU_SPLIT);
     else if (ep.swiglu) PSAM_V4(false, EPI_SWIGLU);
     else if (ep.accumulate) PSAM_V4(false, EPI_ACC);
@@ -322,22 +295,14 @@ __device__ __forceinline__ void epi_chunk_v4_dispatch(float* stg, const uint32_t
 }
 
 
-// Shared epilogue of the 1-CTA and 2-CTA kernels: TMEM -> registers (thread = row) -> per-warp smem transpose ->
-// coalesced global accesses (lane = column: every store/load/red touches one contiguous 128-byte row segment).
-__device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const GemmEpilogue& ep, unsigned char* smem_aligned,
-                                              uint32_t tmem_base, uint32_t tmem_full_bar_addr, int warp, int lane, int m_tile,
-                                              int n_tile, int b1, int b2, int split, int num_kb, int BN,
-                                              int epq = GEMM_EPI_PER_QUARTER, uint32_t full_parity = 0u, int first_warp = 2) {
-        const int quarter = warp & 3;  // TMEM lanes [32*quarter, 32*quarter+32) are accessible to this warp
+
+// Epilogue of one 128 x BN tile from the staged fp32 accumulators `tile` (row pitch `pitch` floats).  Warp w of the
+// eight consumer warps owns rows [32 (w % 4), +32) and the interleaved 32-column chunks c = w / 4, w / 4 + 2, ...
+__device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const GemmEpilogue& ep, const float* tile, int pitch, int warp,
+                                              int lane, int m_tile, int n_tile, int b1, int b2, int split, int BN) {
+        const int quarter = warp & 3;
         const int row0 = m_tile * GEMM_BM + quarter * 32;
-        if (num_kb > 0) {
-            mbar_wait(tmem_full_bar_addr, full_parity);
-            tc_fence_after();
-        }
-        // One-shot kernels: all TMA loads have landed and all MMAs have retired, the pipeline stages are free to reuse
-        // (smem_aligned = stage memory).  Persistent kernel: smem_aligned points at a dedicated staging area.
-        float* stg = reinterpret_cast<float*>(smem_aligned) + (warp - first_warp) * (32 * EPI_PITCH);  // 16-byte aligned rows
-        const int ehalf = (warp - first_warp) >> 2;  // the warps of a lane quarter take interleaved 32-column chunks
+        const int ehalf = warp >> 2;
         const long long obase = (long long)b1 * ep.out_b1 + (long long)b2 * ep.out_b2;
         float* out = ep.out_f32 ? ep.out_f32 + obase : nullptr;
         const float* res = (ep.resid && !ep.accumulate) ? ep.resid + obase : nullptr;
@@ -345,17 +310,10 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
         const bool add_bias = ep.bias && split == 0;
         const int nchunks = BN / 32;
 #pragma unroll 1
-        for (int c = ehalf; c < nchunks; c += epq) {
+        for (int c = ehalf; c < nchunks; c += 2) {
             const int col0 = n_tile * BN + c * 32;
             if (col0 >= shape.N) break;
-            uint32_t v[32];
-            if (num_kb > 0) {
-                tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(c * 32), v);
-                tmem_ld_wait();
-            } else {
-#pragma unroll
-                for (int t = 0; t < 32; ++t) v[t] = 0u;
-            }
+            const float* stg = tile + quarter * 32 * pitch + c * 32;
             if (ep.rd_out) {
                 // fused "masks = hyper_in @ upscaled^T" (mask_decoder.py:176): thread = row, the activated row chunk is
                 // dotted with the rd_c hyper vectors and accumulated with one atomic per (row, c); the 32768 x 256
@@ -370,7 +328,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
                 for (int t = 0; t < 32; ++t) {
                     const int cidx = col0 + t;
                     if (cidx < shape.N) {
-                        const float x = apply_act(fmaf(__uint_as_float(v[t]), ep.alpha, add_bias ? ep.bias[cidx] : 0.f), ep.act);
+                        const float x = apply_act(fmaf(stg[lane * pitch + t], ep.alpha, add_bias ? ep.bias[cidx] : 0.f), ep.act);
 #pragma unroll
                         for (int cc = 0; cc < 8; ++cc)
                             if (cc < ep.rd_c) accd[cc] = fmaf(x, wz[cc * shape.N + cidx], accd[cc]);
@@ -386,15 +344,11 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
             }
             if (ep.vec4 && col0 + 32 <= shape.N) {
                 if (ep.swiglu || ep.accumulate || ep.act == ACT_NONE)
-                    epi_chunk_v4_dispatch<ACT_NONE>(stg, v, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
-                else if (ep.act == ACT_GELU) epi_chunk_v4_dispatch<ACT_GELU>(stg, v, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
-                else epi_chunk_v4_dispatch<ACT_RELU>(stg, v, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
+                    epi_chunk_v4_dispatch<ACT_NONE>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
+                else if (ep.act == ACT_GELU) epi_chunk_v4_dispatch<ACT_GELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
+                else epi_chunk_v4_dispatch<ACT_RELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
                 continue;
             }
-            __syncwarp();
-#pragma unroll
-            for (int t = 0; t < 32; ++t) stg[lane * 33 + t] = __uint_as_float(v[t]);
-            __syncwarp();
             const int col = col0 + lane;
             const bool col_ok = col < shape.N;
             if (ep.gmax) {
@@ -404,14 +358,14 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
                 float m = __int_as_float(0xff800000);
 #pragma unroll 8
                 for (int r = 0; r < 32; ++r)
-                    if (row0 + r < shape.M) m = fmaxf(m, fmaf(stg[r * 33 + lane], ep.alpha, bvm));
+                    if (row0 + r < shape.M) m = fmaxf(m, fmaf(stg[r * pitch + lane], ep.alpha, bvm));
                 if (col_ok && row0 < shape.M) atomic_max_f32(ep.gmax + (long long)(row0 / ep.group_rows) * ep.ld_gmax + col, m);
                 if (out == nullptr && ohi == nullptr) continue;
             }
             if (ohi == nullptr) {
                 const float bv = (add_bias && col_ok) ? ep.bias[col] : 0.f;
-#define PSAM_EPI_F32(A, R, C) epi_rows_f32<A, R, C>(stg, lane, row0, shape.M, col, col_ok, ep.alpha, bv, out, res, ep.ldo)
-                if (ep.swiglu) epi_rows_swiglu(stg, lane, row0, shape.M, col, col_ok, ep.alpha, bv, out, ep.ldo);
+#define PSAM_EPI_F32(A, R, C) epi_rows_f32<A, R, C>(stg, pitch, lane, row0, shape.M, col, col_ok, ep.alpha, bv, out, res, ep.ldo)
+                if (ep.swiglu) epi_rows_swiglu(stg, pitch, lane, row0, shape.M, col, col_ok, ep.alpha, bv, out, ep.ldo);
                 else if (ep.accumulate) PSAM_EPI_F32(ACT_NONE, false, true);
                 else if (res) {
                     if (ep.act == ACT_NONE) PSAM_EPI_F32(ACT_NONE, true, false);
@@ -426,7 +380,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
             } else {
                 const float* bias = add_bias ? ep.bias : nullptr;
                 const bool va = ((ep.ldo_s | ep.out_plane | ep.outs_b1 | ep.outs_b2) & 1) == 0;
-#define PSAM_EPI_SP(A, R, F) epi_rows_split<A, R, F>(stg, lane, row0, shape.M, shape.N, col0, ep.alpha, bias, out, res, ep.ldo, ohi, ep.out_plane, ep.ldo_s, va)
+#define PSAM_EPI_SP(A, R, F) epi_rows_split<A, R, F>(stg, pitch, lane, row0, shape.M, shape.N, col0, ep.alpha, bias, out, res, ep.ldo, ohi, ep.out_plane, ep.ldo_s, va)
 #define PSAM_EPI_SP_ACT(R, F)                                   \
     if (ep.act == ACT_NONE) PSAM_EPI_SP(ACT_NONE, R, F);        \
     else if (ep.act == ACT_GELU) PSAM_EPI_SP(ACT_GELU, R, F);   \
@@ -442,175 +396,46 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
         }
 }
 
-// BK = 64: rows of 128 B, SWIZZLE_128B.  BK = 32: rows of 64 B, SWIZZLE_64B - half-size stages, twice as many of them
-// in flight (finer-grained pipeline; the wide-tile throughput configuration otherwise has only 2 stages).
-// EPQ = epilogue warps per TMEM lane quarter, RES = CTAs of this kernel that must fit one SM.  <256, 2, 32, 2, 2> is the
-// DUAL-RESIDENT configuration of the throughput policy: 97 KB of shared memory, 256 TMEM columns and 320 threads per CTA,
-// so two CTAs (usually of different clouds' launches) share an SM and one's TMA ramp-up / epilogue overlaps the other's
-// MMAs - with one 197 KB CTA per SM the tensor pipe idles for about half of every CTA's lifetime
-// (profiles/r01_gemm_qkv_bn256_ncu_full.md: 49.6 % active).
-template <int MAXBN, int STAGES, int BK, int EPQ = GEMM_EPI_PER_QUARTER, int RES = 1>
-__global__ void __launch_bounds__(gemm_threads(EPQ), RES)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const __grid_constant__ CUtensorMap tmap_bmc, const GemmShape shape, const GemmEpilogue ep) {
-    pdl_launch_dependents();
-    using S = GemmSmem<MAXBN, STAGES, BK>;
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t full_bar[STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
+// Named barrier of the 256 consumer threads (the TMA warp does not take part).
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-    const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    unsigned char* smem_aligned = smem_dyn + (smem_base - smem_u32(smem_dyn));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n_tile = blockIdx.x, m_tile = blockIdx.y;
-    const int z = blockIdx.z;
-    const int split = z % shape.split_k;
-    const int bz = z / shape.split_k;
-    const int b1 = bz % shape.nb1, b2 = bz / shape.nb1;
-    const int BN = shape.bn;
-    const uint32_t cm = (uint32_t)shape.cm;                       // CTAs sharing the W tile (cluster along M)
-    const uint32_t crank = cm > 1 ? cluster_ctarank() : 0u;
-    const uint16_t cmask = (uint16_t)((1u << cm) - 1u);
-
-    const int kb_total = (shape.K + BK - 1) / BK;
-    const int kb_per = (kb_total + shape.split_k - 1) / shape.split_k;
-    const int kb_begin = split * kb_per;
-    const int kb_end = min(kb_total, kb_begin + kb_per);
-    const int num_kb = max(0, kb_end - kb_begin);
-    const bool lo_pass = shape.passes == 3;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_b);
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), cm);  // every CTA of the cluster writes into this stage
-        }
-        mbar_init(smem_u32(&tmem_full_bar), 1);
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), S::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    if (cm > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast / remote arrive
-    pdl_wait();  // everything above is independent of the previous kernel; its outputs are read only below
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        // lane 0 streams the A tiles, lane 1 the W tiles; the hi and lo planes of a tile arrive with ONE
-        // 3-D box (64 x rows x 2 planes) - TMA cost is dominated by a fixed per-operation overhead.
-        if (lane < 2) {
-            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(S::A_TILE + BN * BK * 2);
-            if (lane == 1 && cm == 1)
-                for (int i = 0; i < shape.prefetch && i < num_kb; ++i) tma_prefetch_l2_5d(&tmap_b, (kb_begin + i) * BK, n_tile * BN, 0, b1, b2);
-            for (int i = 0; i < num_kb; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-                mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1u);
-                const uint32_t fb = smem_u32(&full_bar[s]);
-                const uint32_t sa = smem_base + s * S::STAGE;
-                const int k0 = (kb_begin + i) * BK;
-                if (lane == 0) {
-                    mbar_arrive_expect_tx(fb, stage_bytes);
-                    tma_load_5d(sa, &tmap_a, fb, k0, m_tile * GEMM_BM, 0, b1, b2);
-                } else if (cm == 1) {
-                    // the W tile is read from DRAM exactly once per step: ask L2 for the tile GEMM_PREFETCH k-blocks ahead
-                    if (shape.prefetch > 0 && i + shape.prefetch < num_kb)
-                        tma_prefetch_l2_5d(&tmap_b, (kb_begin + i + shape.prefetch) * BK, n_tile * BN, 0, b1, b2);
-                    tma_load_5d(sa + 2 * S::A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
-                } else {
-                    // this CTA fetches rows [crank*BN/cm, (crank+1)*BN/cm) of the W tile once and multicasts them
-                    // into the same stage of every CTA of the cluster (hi and lo planes separately)
-                    const int rows = BN / (int)cm;
-                    const uint32_t off = crank * (uint32_t)rows * 128u;
-                    tma_load_5d_mc(sa + 2 * S::A_TILE + off, &tmap_bmc, fb, k0, n_tile * BN + (int)crank * rows, 0, b1, b2, cmask);
-                    if (lo_pass)
-                        tma_load_5d_mc(sa + 2 * S::A_TILE + BN * BK * 2 + off, &tmap_bmc, fb, k0, n_tile * BN + (int)crank * rows, 1, b1, b2, cmask);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        const uint32_t idesc = umma_idesc_bf16(GEMM_BM, BN);
-        for (int i = 0; i < num_kb; ++i) {
-            const int s = i % STAGES;
-            const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-            mbar_wait(smem_u32(&full_bar[s]), ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sa = smem_base + s * S::STAGE;
-                const uint64_t a_hi = umma_desc_k<BK>(sa);
-                const uint64_t a_lo = umma_desc_k<BK>(sa + S::A_TILE);
-                const uint64_t b_hi = umma_desc_k<BK>(sa + 2 * S::A_TILE);
-                const uint64_t b_lo = umma_desc_k<BK>(sa + 2 * S::A_TILE + BN * BK * 2);
+// One k-block of the split-bf16 product into the warpgroup's 64 x BN accumulator: 4 k-steps per pass.
+template <int BN>
+__device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_hi_addr, uint32_t a_lo_addr, uint32_t b_hi_addr,
+                                            uint32_t b_lo_addr, bool lo_pass) {
+    const uint64_t a_hi = gmma_desc_k(a_hi_addr), b_hi = gmma_desc_k(b_hi_addr);
 #pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)(k * 2);  // 16 bf16 = 32 B = 2 x 16-byte units
-                    umma_bf16(tmem_base, a_hi + adv, b_hi + adv, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                }
-                if (lo_pass) {
+    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
+    if (lo_pass) {
+        const uint64_t a_lo = gmma_desc_k(a_lo_addr), b_lo = gmma_desc_k(b_lo_addr);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t adv = (uint64_t)(k * 2);
-                        umma_bf16(tmem_base, a_lo + adv, b_hi + adv, idesc, 1u);
-                    }
+        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t adv = (uint64_t)(k * 2);
-                        umma_bf16(tmem_base, a_hi + adv, b_lo + adv, idesc, 1u);
-                    }
-                }
-                if (cm > 1) umma_commit_mc(smem_u32(&empty_bar[s]), cmask);  // release the stage in every CTA of the cluster
-                else umma_commit(smem_u32(&empty_bar[s]));                   // stage reusable once these MMAs retire
-                if (i == num_kb - 1) umma_commit(smem_u32(&tmem_full_bar));  // accumulator complete
-            }
-            __syncwarp();
-        }
-    } else {
-        // ===================== epilogue (warps 2..9) =====================
-        // TMEM -> registers (thread = row) -> per-warp smem transpose -> coalesced global accesses
-        // (lane = column: every store/load/red instruction touches one contiguous 128-byte row segment).
-        gemm_epilogue(shape, ep, smem_aligned, tmem_base, smem_u32(&tmem_full_bar), warp, lane, m_tile, n_tile, b1, b2, split, num_kb, BN, EPQ);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (cm > 1) cluster_sync_all();  // no CTA leaves while peers can still multicast into it or arrive on its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, S::TMEM_COLS);
+        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
     }
 }
 
+// Accumulator fragment of wgmma m64nN (thread = lane of warp w of the warpgroup): register i holds row
+// 16 w + lane / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (lane % 4) + i % 2.
+template <int BN>
+__device__ __forceinline__ void stage_acc(float* tile, int pitch, int row_base, int lane, const float (&acc)[BN / 2]) {
+    const int r = row_base + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(tile + r * pitch + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (r + 8) * pitch + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+}
 
-// ---------------------------------------------------------------------------------------------
-// Two-issuer variant of the one-shot wide-tile kernel (experiment, opt-in: GV_TWO_ISSUERS; see the dispatch for the measurement).
-// One thread issues a tcgen05.mma every ~120 clk at best and a 128 x 256 x 16 MMA (128 clk of tensor time) every 171 clk from
-// shared-memory operands; two issuing threads reach 150.6 clk (tools/mma_issue_probe.cu, also when both accumulate into the
-// SAME tensor-memory accumulator).  So the 12 MMAs of a 64-deep k-block are split between two warps (k-steps 0-1 / 2-3 of
-// each split-bf16 pass).  All MMAs accumulate (the epilogue warps zero the accumulator while the TMA pipeline fills), so no
-// order between the two issuers is required; the fp32 summation order of a k-block is therefore not fixed (like split-K).
-//   warp 0: TMA producer, warps 1-2: MMA issuers, warp 3: idle, warps 4-15: epilogue (three per TMEM lane quarter).
-// ---------------------------------------------------------------------------------------------
-constexpr int DUO_EPQ = 3;
-constexpr int DUO_THREADS = 128 + 128 * DUO_EPQ;
-
-template <int MAXBN, int STAGES>
-__global__ void __launch_bounds__(DUO_THREADS, 1)
-gemm_tc_duo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmShape shape,
-                   const GemmEpilogue ep) {
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmShape shape,
+                  const GemmEpilogue ep) {
     pdl_launch_dependents();
-    constexpr int BK = 64;
-    using S = GemmSmem<MAXBN, STAGES, BK>;
+    using S = GemmSmem<BN, STAGES>;
     extern __shared__ unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[STAGES];
     __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar, acc_zero_bar;
-    __shared__ uint32_t tmem_base_smem;
 
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
     unsigned char* smem_aligned = smem_dyn + (smem_base - smem_u32(smem_dyn));
@@ -620,276 +445,80 @@ gemm_tc_duo_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     const int split = z % shape.split_k;
     const int bz = z / shape.split_k;
     const int b1 = bz % shape.nb1, b2 = bz / shape.nb1;
-    const int BN = shape.bn;
-    const int kb_total = (shape.K + BK - 1) / BK;
+
+    const int kb_total = (shape.K + GEMM_BK - 1) / GEMM_BK;
     const int kb_per = (kb_total + shape.split_k - 1) / shape.split_k;
     const int kb_begin = split * kb_per;
     const int num_kb = max(0, min(kb_total, kb_begin + kb_per) - kb_begin);
     const bool lo_pass = shape.passes == 3;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 2);   // both issuers release a stage
+            mbar_init(smem_u32(&empty_bar[s]), 2);  // one arrival per consumer warpgroup
         }
-        mbar_init(smem_u32(&tmem_full_bar), 2);      // both issuers complete the accumulator
-        mbar_init(smem_u32(&acc_zero_bar), 4 * DUO_EPQ);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), S::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    pdl_wait();
+    pdl_wait();  // everything above is independent of the previous kernel; its outputs are read only below
 
-    if (warp == 0) {
-        if (lane < 2) {
-            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(S::A_TILE + BN * BK * 2);
+    if (warp == 8) {
+        // ===================== TMA producer: the hi and lo planes of a tile arrive with ONE 3-D box =====================
+        if (lane == 0) {
+            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(GEMM_A_TILE + S::B_TILE);
             for (int i = 0; i < num_kb; ++i) {
                 const int s = i % STAGES;
-                const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-                mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1u);
+                mbar_wait(smem_u32(&empty_bar[s]), ((uint32_t)(i / STAGES) & 1u) ^ 1u);
                 const uint32_t fb = smem_u32(&full_bar[s]);
                 const uint32_t sa = smem_base + s * S::STAGE;
-                const int k0 = (kb_begin + i) * BK;
-                if (lane == 0) {
-                    mbar_arrive_expect_tx(fb, stage_bytes);
-                    tma_load_5d(sa, &tmap_a, fb, k0, m_tile * GEMM_BM, 0, b1, b2);
-                } else {
-                    tma_load_5d(sa + 2 * S::A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
-                }
+                const int k0 = (kb_begin + i) * GEMM_BK;
+                mbar_arrive_expect_tx(fb, stage_bytes);
+                tma_load_5d(sa, &tmap_a, fb, k0, m_tile * GEMM_BM, 0, b1, b2);
+                tma_load_5d(sa + 2 * GEMM_A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
             }
         }
-    } else if (warp == 1 || warp == 2) {
-        // ===================== MMA issuers: k-steps {0,1} (warp 1) / {2,3} (warp 2) of every pass =====================
-        const uint32_t idesc = umma_idesc_bf16(GEMM_BM, BN);
-        const int k_first = (warp - 1) * 2;
-        if (num_kb > 0) {
-            mbar_wait(smem_u32(&acc_zero_bar), 0);  // the accumulator has been zeroed
-            tc_fence_after();
-        }
-        for (int i = 0; i < num_kb; ++i) {
-            const int s = i % STAGES;
-            const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-            mbar_wait(smem_u32(&full_bar[s]), ph);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t sa = smem_base + s * S::STAGE;
-                const uint64_t a_hi = umma_desc_k<BK>(sa), a_lo = umma_desc_k<BK>(sa + S::A_TILE);
-                const uint64_t b_hi = umma_desc_k<BK>(sa + 2 * S::A_TILE), b_lo = umma_desc_k<BK>(sa + 2 * S::A_TILE + BN * BK * 2);
-#pragma unroll
-                for (int k = 0; k < 2; ++k) umma_bf16(tmem_base, a_hi + 2 * (k_first + k), b_hi + 2 * (k_first + k), idesc, 1u);
-                if (lo_pass) {
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) umma_bf16(tmem_base, a_lo + 2 * (k_first + k), b_hi + 2 * (k_first + k), idesc, 1u);
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) umma_bf16(tmem_base, a_hi + 2 * (k_first + k), b_lo + 2 * (k_first + k), idesc, 1u);
-                }
-                umma_commit(smem_u32(&empty_bar[s]));
-                if (i == num_kb - 1) umma_commit(smem_u32(&tmem_full_bar));
-            }
-            __syncwarp();
-        }
-    } else if (warp >= 4) {
-        // ===================== epilogue warps: zero the accumulator, later drain it =====================
-        if (num_kb > 0) {
-            const uint32_t q = (uint32_t)((warp & 3) * 32) << 16;
-            uint32_t zr[32];
-#pragma unroll
-            for (int t = 0; t < 32; ++t) zr[t] = 0u;
-            for (int c = (warp - 4) >> 2; c < BN / 32; c += DUO_EPQ) tmem_st_32x32(tmem_base + q + (uint32_t)(c * 32), zr);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&acc_zero_bar));
-        }
-        gemm_epilogue(shape, ep, smem_aligned, tmem_base, smem_u32(&tmem_full_bar), warp, lane, m_tile, n_tile, b1, b2, split, num_kb, BN,
-                      DUO_EPQ, 0u, 4);
+        return;
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, S::TMEM_COLS);
-    }
-}
-
-template <int MAXBN, int STAGES>
-static int launch_gemm_duo(const CUtensorMap& ma, const CUtensorMap& mb, const GemmShape& sh, const GemmEpilogue& ep, cudaStream_t stream) {
-    auto kern = gemm_tc_duo_kernel<MAXBN, STAGES>;
-    using S = GemmSmem<MAXBN, STAGES, 64>;
-    PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    const dim3 grid((unsigned)ceil_div(sh.N, sh.bn), (unsigned)ceil_div(sh.M, GEMM_BM), (unsigned)(sh.nb1 * sh.nb2 * sh.split_k));
-    PSAM_CUDA_TRY(psam::launch(kern, grid, dim3(DUO_THREADS), (size_t)S::TOTAL, stream, ma, mb, sh, ep));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Persistent variant: grid = min(tiles, SMs); every CTA walks the linear tile index (m fastest, so the CTAs running at the
-// same time share W tiles through L2) with a stride of gridDim.x.  The accumulator is DOUBLE-BUFFERED in tensor memory
-// (2 x ACC_COLS columns): the epilogue warps drain tile i while the MMA warp already accumulates tile i+1, and the TMA
-// producer never stops - the shared-memory stage ring runs across tile boundaries.  The one-shot kernel above pays
-// TMEM allocation, barrier setup, pipeline fill and the whole epilogue once per 128 x BN tile with the tensor pipe idle;
-// here they are paid once per CTA, or hidden.  The epilogue has its own staging memory (the stage ring is never idle), so
-// the wide-tile configuration uses BK = 32 stages (48 KB) x 4 with four epilogue warps.
-// ---------------------------------------------------------------------------------------------
-template <int MAXBN, int STAGES, int BK, int EPQ>
-__global__ void __launch_bounds__(gemm_threads(EPQ), 1)
-gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmShape shape,
-                       const GemmEpilogue ep) {
-    pdl_launch_dependents();
-    using S = GemmSmem<MAXBN, STAGES, BK>;
-    constexpr int ACC_COLS = S::TMEM_COLS;
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t full_bar[STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t acc_full[2], acc_empty[2];
-    __shared__ uint32_t tmem_base_smem;
-
-    const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    unsigned char* smem_aligned = smem_dyn + (smem_base - smem_u32(smem_dyn));
-    unsigned char* staging = smem_aligned + STAGES * S::STAGE;  // 4*EPQ warps x 32 x EPI_PITCH floats
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int BN = shape.bn;
-    const int MT = ceil_div(shape.M, GEMM_BM), NT = ceil_div(shape.N, BN);
-    const int total = MT * NT * shape.nb1 * shape.nb2 * shape.split_k;
-    const int kb_total = (shape.K + BK - 1) / BK;
-    const int kb_per = (kb_total + shape.split_k - 1) / shape.split_k;
-    const bool lo_pass = shape.passes == 3;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_b);
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(smem_u32(&acc_full[b]), 1);
-            mbar_init(smem_u32(&acc_empty[b]), 4 * EPQ);  // one arrival per epilogue warp
-        }
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), 2 * ACC_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    pdl_wait();
-
-    // tile -> (m_tile, n_tile, b1, b2, split) and its k-block range; identical in the three roles
-    auto decode = [&](int tile, int& m_tile, int& n_tile, int& b1, int& b2, int& split, int& kb_begin, int& num_kb) {
-        m_tile = tile % MT;
-        n_tile = (tile / MT) % NT;
-        const int z = tile / (MT * NT);
-        split = z % shape.split_k;
-        const int bz = z / shape.split_k;
-        b1 = bz % shape.nb1, b2 = bz / shape.nb1;
-        kb_begin = split * kb_per;
-        num_kb = max(0, min(kb_total, kb_begin + kb_per) - kb_begin);
-    };
-
-    if (warp == 0) {
-        // ===================== TMA producer: lane 0 streams A, lane 1 streams W =====================
-        if (lane < 2) {
-            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(S::A_TILE + BN * BK * 2);
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-                int m_tile, n_tile, b1, b2, split, kb_begin, num_kb;
-                decode(tile, m_tile, n_tile, b1, b2, split, kb_begin, num_kb);
-                for (int i = 0; i < num_kb; ++i, ++it) {
-                    const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-                    mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1u);
-                    const uint32_t fb = smem_u32(&full_bar[s]);
-                    const uint32_t sa = smem_base + s * S::STAGE;
-                    const int k0 = (kb_begin + i) * BK;
-                    if (lane == 0) {
-                        mbar_arrive_expect_tx(fb, stage_bytes);
-                        tma_load_5d(sa, &tmap_a, fb, k0, m_tile * GEMM_BM, 0, b1, b2);
-                    } else {
-                        tma_load_5d(sa + 2 * S::A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        const uint32_t idesc = umma_idesc_bf16(GEMM_BM, BN);
-        uint32_t it = 0, acc_it = 0;
-        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-            int m_tile, n_tile, b1, b2, split, kb_begin, num_kb;
-            decode(tile, m_tile, n_tile, b1, b2, split, kb_begin, num_kb);
-            if (num_kb == 0) continue;
-            const uint32_t ab = acc_it & 1u;
-            mbar_wait(smem_u32(&acc_empty[ab]), ((acc_it >> 1) & 1u) ^ 1u);  // the epilogue has drained this accumulator
-            tc_fence_after();
-            const uint32_t d_acc = tmem_base + ab * (uint32_t)ACC_COLS;
-            for (int i = 0; i < num_kb; ++i, ++it) {
-                const uint32_t s = it % STAGES, ph = (it / STAGES) & 1u;
-                mbar_wait(smem_u32(&full_bar[s]), ph);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t sa = smem_base + s * S::STAGE;
-                    const uint64_t a_hi = umma_desc_k<BK>(sa);
-                    const uint64_t a_lo = umma_desc_k<BK>(sa + S::A_TILE);
-                    const uint64_t b_hi = umma_desc_k<BK>(sa + 2 * S::A_TILE);
-                    const uint64_t b_lo = umma_desc_k<BK>(sa + 2 * S::A_TILE + BN * BK * 2);
+    // ===================== consumer warpgroups =====================
+    const int wg = warp >> 2;
+    float acc[BN / 2];
 #pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) umma_bf16(d_acc, a_hi + 2 * k, b_hi + 2 * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    if (lo_pass) {
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) umma_bf16(d_acc, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) umma_bf16(d_acc, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-                    }
-                    umma_commit(smem_u32(&empty_bar[s]));
-                    if (i == num_kb - 1) umma_commit(smem_u32(&acc_full[ab]));
-                }
-                __syncwarp();
-            }
-            ++acc_it;
-        }
-    } else {
-        // ===================== epilogue warps =====================
-        uint32_t acc_it = 0;
-        for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-            int m_tile, n_tile, b1, b2, split, kb_begin, num_kb;
-            decode(tile, m_tile, n_tile, b1, b2, split, kb_begin, num_kb);
-            const uint32_t ab = acc_it & 1u;
-            gemm_epilogue(shape, ep, staging, tmem_base + ab * (uint32_t)ACC_COLS, smem_u32(&acc_full[ab]), warp, lane, m_tile, n_tile,
-                          b1, b2, split, num_kb, BN, EPQ, (acc_it >> 1) & 1u);
-            if (num_kb > 0) {
-                tc_fence_before();  // this warp's tcgen05.ld of the accumulator are complete
-                __syncwarp();
-                if (lane == 0) mbar_arrive(smem_u32(&acc_empty[ab]));
-                ++acc_it;
-            }
-        }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < num_kb; ++i) {
+        const int s = i % STAGES;
+        mbar_wait(smem_u32(&full_bar[s]), (uint32_t)(i / STAGES) & 1u);
+        const uint32_t sa = smem_base + s * S::STAGE + wg * (GEMM_A_TILE / 2);  // this warpgroup's 64 rows
+        const uint32_t sb = smem_base + s * S::STAGE + 2 * GEMM_A_TILE;
+        fence_acc(acc);
+        wgmma_fence();
+        gemm_kblock<BN>(acc, sa, sa + GEMM_A_TILE, sb, sb + S::B_TILE, lo_pass);
+        wgmma_commit();
+        wgmma_wait<1>();  // the k-block before this one has retired: release its stage
+        fence_acc(acc);
+        if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(i - 1) % STAGES]));
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 2 * ACC_COLS);
-    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    consumers_sync();  // every wgmma of both warpgroups has read its stage: the stage memory becomes the output tile
+    float* tile = reinterpret_cast<float*>(smem_aligned);
+    stage_acc<BN>(tile, S::PITCH, wg * 64 + (warp & 3) * 16, lane, acc);
+    consumers_sync();
+    gemm_epilogue(shape, ep, tile, S::PITCH, warp, lane, m_tile, n_tile, b1, b2, split, BN);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Row-complete GEMM with LayerNorm + GELU in the epilogue (mini-PointNet conv2[0..2], pc_sam/model/common.py:491-495):
 //     Y = GELU(LayerNorm(A W^T + gbias[row / group_rows]))  ->  split-bf16
-// A CTA owns 128 rows x the FULL output width N = 256 NH (NH = 1 or 2 accumulators of 256 TMEM columns), so the row statistics
-// never leave the SM and the fp32 pre-activation (32768 x 512 floats = 64 MB per cloud, written by the GEMM and read back by
-// the LayerNorm kernel before) never reaches memory.  K <= 128: the A tile (both k-blocks, hi + lo = 64 KB) stays in shared
-// memory while W streams through one 128 KB buffer, one 256-row half at a time (W is L2-resident: every CTA reads the same 256 KB).
-// Persistent over the m-tiles.  warp 0: TMA, warp 1: MMA, warps 2-17: epilogue (four per TMEM lane quarter, N / 4 columns each):
-// pass 1 reads the accumulator once for shifted sums (Chan's parallel variance across the four parts of a row), pass 2 reads
-// it again, normalises, applies GELU and stores both bf16 planes straight from registers (64 contiguous bytes per thread).
+// A CTA owns 128 rows (warpgroup g: rows 64 g .. 64 g + 63) and computes each row over the FULL output width N = 256 NH,
+// so the row statistics never leave the warp (a warp holds 16 whole rows; the four lanes of a quad share a row) and the
+// fp32 pre-activation never reaches memory.  K <= 128: the A tile (both k-blocks, hi + lo = 64 KB) stays in shared memory
+// while W sits in one 128 KB buffer, 256 rows at a time.  The registers hold one 64 x 256 accumulator per warpgroup, so
+//   NH = 1: W is loaded once per CTA and stays resident; each tile is one product, exact two-pass statistics in registers;
+//   NH = 2: the halves are computed in the order 0, 1, 0 - half 0 for its statistics only, half 1 for its statistics and
+//           output (the two halves' (mean, M2) combined as in Chan et al.), half 0 again for its output.
+// Persistent over the m-tiles.  warps 0-7: consumers, warp 8: TMA.
 // ---------------------------------------------------------------------------------------------
 struct RowLnParams {
     int M, N, K, passes;
@@ -904,341 +533,168 @@ struct RowLnParams {
     long long out_plane, ldo_s;
 };
 
-constexpr int RL_THREADS = 576;  // TMA warp, MMA warp, 16 epilogue warps (four threads per row, N / 4 columns each)
 constexpr int RL_A_TILE = 128 * 64 * 2;                  // one plane of one k-block of A
 constexpr int RL_W_TILE = 256 * 64 * 2;                  // one plane of one k-block of a W half
 constexpr int RL_SMEM = 2 * 2 * RL_A_TILE + 2 * 2 * RL_W_TILE + 1024;  // A: 2 k-blocks x (hi, lo); W half: 2 k-blocks x (hi, lo)
 
-__global__ void __launch_bounds__(RL_THREADS, 1)
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_rowln_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w, const RowLnParams p) {
     pdl_launch_dependents();
     extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t a_full, a_empty, w_full, w_empty, acc_full, acc_empty;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ float2 s_part[2][4][128];  // [tile parity][part][row]: (mean, M2) of each quarter of a row
+    __shared__ __align__(8) uint64_t a_full, a_empty, w_full, w_empty;
 
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
     const uint32_t sA = smem_base, sW = smem_base + 4 * RL_A_TILE;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int MT = ceil_div(p.M, GEMM_BM);
-    const int NH = p.N / 256;                      // accumulators (halves of the row)
+    const int NH = p.N / 256;                      // 256-column halves of the row
     const int KB = ceil_div(p.K, 64);              // k-blocks (1 or 2)
     const bool lo_pass = p.passes == 3;
     const uint32_t planes = lo_pass ? 2u : 1u;
+    const bool resident = NH == 1;                 // W loaded once
+    const int steps = NH == 1 ? 1 : 3;             // W halves per tile: 0 | 0, 1, 0
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
         mbar_init(smem_u32(&a_full), 1);
-        mbar_init(smem_u32(&a_empty), 1);
+        mbar_init(smem_u32(&a_empty), 2);
         mbar_init(smem_u32(&w_full), 1);
-        mbar_init(smem_u32(&w_empty), 1);
-        mbar_init(smem_u32(&acc_full), 1);
-        mbar_init(smem_u32(&acc_empty), 16);
+        mbar_init(smem_u32(&w_empty), 2);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
+            auto load_w = [&](int h) {
+                mbar_arrive_expect_tx(smem_u32(&w_full), planes * (uint32_t)(KB * RL_W_TILE));
+                for (int kb = 0; kb < KB; ++kb)  // one 3-D box per k-block: 64 x 256 rows x {hi, lo}
+                    tma_load_5d(sW + kb * 2 * RL_W_TILE, &tmap_w, smem_u32(&w_full), kb * 64, h * 256, 0, 0, 0);
+            };
+            if (resident) load_w(0);
             uint32_t it = 0, wit = 0;
             for (int tile = blockIdx.x; tile < MT; tile += gridDim.x, ++it) {
                 mbar_wait(smem_u32(&a_empty), (it & 1u) ^ 1u);
                 mbar_arrive_expect_tx(smem_u32(&a_full), planes * (uint32_t)(KB * RL_A_TILE));
-                for (int kb = 0; kb < KB; ++kb)  // one 3-D box per k-block: 64 x 128 rows x {hi, lo}
+                for (int kb = 0; kb < KB; ++kb)
                     tma_load_5d(sA + kb * 2 * RL_A_TILE, &tmap_a, smem_u32(&a_full), kb * 64, tile * GEMM_BM, 0, 0, 0);
-                for (int h = 0; h < NH; ++h, ++wit) {
-                    mbar_wait(smem_u32(&w_empty), (wit & 1u) ^ 1u);
-                    mbar_arrive_expect_tx(smem_u32(&w_full), planes * (uint32_t)(KB * RL_W_TILE));
-                    for (int kb = 0; kb < KB; ++kb)
-                        tma_load_5d(sW + kb * 2 * RL_W_TILE, &tmap_w, smem_u32(&w_full), kb * 64, h * 256, 0, 0, 0);
+                if (!resident) {
+                    for (int st = 0; st < steps; ++st, ++wit) {
+                        mbar_wait(smem_u32(&w_empty), (wit & 1u) ^ 1u);
+                        load_w(st == 1 ? 1 : 0);
+                    }
                 }
             }
         }
-    } else if (warp == 1) {
-        const uint32_t idesc = umma_idesc_bf16(GEMM_BM, 256);
-        uint32_t it = 0, wit = 0;
-        for (int tile = blockIdx.x; tile < MT; tile += gridDim.x, ++it) {
-            mbar_wait(smem_u32(&acc_empty), (it & 1u) ^ 1u);  // the epilogue has drained the accumulators of the previous tile
-            mbar_wait(smem_u32(&a_full), it & 1u);
-            tc_fence_after();
-            for (int h = 0; h < NH; ++h, ++wit) {
-                mbar_wait(smem_u32(&w_full), wit & 1u);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t d = tmem_base + (uint32_t)(h * 256);
-                    for (int kb = 0; kb < KB; ++kb) {
-                        const uint32_t sa = sA + kb * 2 * RL_A_TILE, sw = sW + kb * 2 * RL_W_TILE;
-                        const uint64_t a_hi = umma_desc_k_sw128(sa), a_lo = umma_desc_k_sw128(sa + RL_A_TILE);
-                        const uint64_t b_hi = umma_desc_k_sw128(sw), b_lo = umma_desc_k_sw128(sw + RL_W_TILE);
+        return;
+    }
+
+    const int wg = warp >> 2;
+    const int rw = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // first of this thread's two rows in the tile (second: + 8)
+    const int cq = 2 * (lane & 3);
+    const float inv_half = 1.0f / 256.0f;
+    uint32_t it = 0, wit = 0;
+    for (int tile = blockIdx.x; tile < MT; tile += gridDim.x, ++it) {
+        mbar_wait(smem_u32(&a_full), it & 1u);
+        int rows[2] = {tile * GEMM_BM + rw, tile * GEMM_BM + rw + 8};
+        const float* gb[2];
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) umma_bf16(d, a_hi + 2 * k, b_hi + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                        if (lo_pass) {
+        for (int q = 0; q < 2; ++q) gb[q] = (p.gbias && rows[q] < p.M) ? p.gbias + (long long)(rows[q] / p.group_rows) * p.ld_gbias : nullptr;
+        float mean0[2] = {0.f, 0.f}, m2_0[2] = {0.f, 0.f}, mean[2], rstd[2];
+        for (int st = 0; st < steps; ++st) {
+            const int h = st == 1 ? 1 : 0;
+            if (!resident || it == 0) mbar_wait(smem_u32(&w_full), resident ? 0u : (wit & 1u));
+            float acc[128];
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
+            for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+            fence_acc(acc);
+            wgmma_fence();
 #pragma unroll
-                            for (int k = 0; k < 4; ++k) umma_bf16(d, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-                        }
-                    }
-                    umma_commit(smem_u32(&w_empty));                       // this W half may be overwritten
-                    if (h == NH - 1) {
-                        umma_commit(smem_u32(&a_empty));                   // the A tile too
-                        umma_commit(smem_u32(&acc_full));
-                    }
-                }
-                __syncwarp();
+            for (int kb = 0; kb < 2; ++kb) {
+                if (kb == KB) break;
+                const uint32_t sa = sA + kb * 2 * RL_A_TILE + wg * (RL_A_TILE / 2), sw = sW + kb * 2 * RL_W_TILE;
+                gemm_kblock<256>(acc, sa, sa + RL_A_TILE, sw, sw + RL_W_TILE, lo_pass);
             }
-        }
-    } else {
-        // ===================== epilogue: thread = (row, quarter of the row's columns) =====================
-        const int quarter = warp & 3, part = (warp - 2) >> 2;  // four warps per TMEM lane quarter, one per column part
-        const int r = quarter * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(quarter * 32) << 16;
-        const int cols_part = p.N / 4;                           // 64 or 128 columns per thread
-        const int col_base = part * cols_part;                   // first global column of this thread
-        const int c_count = cols_part / 32;                      // 32-column chunks
-        const uint32_t t_acc = tmem_base + lane_off + (uint32_t)col_base;  // accumulator h occupies TMEM columns [256 h, 256 h + 256)
-        const float inv_n = 1.0f / (float)p.N;
-        const float n_part = (float)cols_part;
-        uint32_t it = 0;
-        for (int tile = blockIdx.x; tile < MT; tile += gridDim.x, ++it) {
-            const int row = tile * GEMM_BM + r;
-            const bool row_ok = row < p.M;
-            const float* gb = (p.gbias && row_ok) ? p.gbias + (long long)(row / p.group_rows) * p.ld_gbias : nullptr;
-            mbar_wait(smem_u32(&acc_full), it & 1u);
-            tc_fence_after();
-            // ---- pass 1: shifted sums of this thread's half of the row ----
-            float shift = 0.f, s1 = 0.f, s2 = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < c_count; ++c) {
-                uint32_t v[32];
-                const int col0 = col_base + c * 32;
-                tmem_ld_32x32(t_acc + (uint32_t)(c * 32), v);
-                tmem_ld_wait();
-                if (c == 0) shift = __uint_as_float(v[0]) + (gb ? gb[col0] : 0.f);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_acc(acc);
+            if (!resident) {
+                ++wit;
+                if ((warp & 3) == 0 && lane == 0) mbar_arrive(smem_u32(&w_empty));  // this W half may be overwritten
+            }
+            if (st == steps - 1 && (warp & 3) == 0 && lane == 0) mbar_arrive(smem_u32(&a_empty));  // the A tile too
+            // pre-activation + group bias, then exact two-pass statistics of this half of the row
+            const int c0 = h * 256;
+            float s1[2] = {0.f, 0.f};
 #pragma unroll
-                for (int t = 0; t < 32; t += 4) {
-                    const float4 g4 = gb ? *reinterpret_cast<const float4*>(gb + col0 + t) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    const float x0 = __uint_as_float(v[t]) + g4.x - shift, x1 = __uint_as_float(v[t + 1]) + g4.y - shift,
-                                x2 = __uint_as_float(v[t + 2]) + g4.z - shift, x3 = __uint_as_float(v[t + 3]) + g4.w - shift;
-                    s1 += (x0 + x1) + (x2 + x3);
-                    s2 = fmaf(x0, x0, fmaf(x1, x1, fmaf(x2, x2, fmaf(x3, x3, s2))));
+            for (int j = 0; j < 32; ++j) {
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const float2 g2 = gb[q] ? *reinterpret_cast<const float2*>(gb[q] + c0 + 8 * j + cq) : make_float2(0.f, 0.f);
+                    acc[4 * j + 2 * q] += g2.x;
+                    acc[4 * j + 2 * q + 1] += g2.y;
+                    s1[q] += acc[4 * j + 2 * q] + acc[4 * j + 2 * q + 1];
                 }
             }
-            const float mean_h = shift + s1 / n_part;
-            const float m2_h = fmaxf(s2 - s1 * s1 / n_part, 0.f);
-            s_part[it & 1u][part][r] = make_float2(mean_h, m2_h);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + quarter) : "memory");  // the four warps of this lane quarter
-            const float2 o0 = s_part[it & 1u][0][r], o1 = s_part[it & 1u][1][r], o2 = s_part[it & 1u][2][r], o3 = s_part[it & 1u][3][r];
-            const float mean = 0.25f * ((o0.x + o1.x) + (o2.x + o3.x));
-            // equal part sizes: M2 = sum M2_p + n_p sum (mean_p - mean)^2   (Chan et al., pairwise combination)
-            const float d0 = o0.x - mean, d1 = o1.x - mean, d2 = o2.x - mean, d3 = o3.x - mean;
-            const float var = (((o0.y + o1.y) + (o2.y + o3.y)) + n_part * ((d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3))) * inv_n;
-            const float rstd = rsqrtf(var + p.eps);
-            // ---- pass 2: normalise, activate, store both planes ----
-            __nv_bfloat16* ohi = p.out_hi + (long long)row * p.ldo_s;
-            __nv_bfloat16* olo = ohi + p.out_plane;
-#pragma unroll 1
-            for (int c = 0; c < c_count; ++c) {
-                uint32_t v[32];
-                const int col0 = col_base + c * 32;
-                tmem_ld_32x32(t_acc + (uint32_t)(c * 32), v);
-                tmem_ld_wait();
-                uint32_t hh[16], ll[16];
+            float mh[2], m2h[2];
 #pragma unroll
-                for (int t = 0; t < 32; t += 4) {
-                    const float4 g4 = gb ? *reinterpret_cast<const float4*>(gb + col0 + t) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    const float4 ga = *reinterpret_cast<const float4*>(p.gamma + col0 + t);
-                    const float4 be = *reinterpret_cast<const float4*>(p.beta + col0 + t);
-                    const float y0 = apply_act(fmaf((__uint_as_float(v[t]) + g4.x - mean) * rstd, ga.x, be.x), p.act);
-                    const float y1 = apply_act(fmaf((__uint_as_float(v[t + 1]) + g4.y - mean) * rstd, ga.y, be.y), p.act);
-                    const float y2 = apply_act(fmaf((__uint_as_float(v[t + 2]) + g4.z - mean) * rstd, ga.z, be.z), p.act);
-                    const float y3 = apply_act(fmaf((__uint_as_float(v[t + 3]) + g4.w - mean) * rstd, ga.w, be.w), p.act);
-                    __nv_bfloat16 h0, l0, h1, l1, h2, l2, h3, l3;
+            for (int q = 0; q < 2; ++q) {
+                mh[q] = quad_sum(s1[q]) * inv_half;
+                float s2 = 0.f;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const float d0 = acc[4 * j + 2 * q] - mh[q], d1 = acc[4 * j + 2 * q + 1] - mh[q];
+                    s2 = fmaf(d0, d0, fmaf(d1, d1, s2));
+                }
+                m2h[q] = quad_sum(s2);
+            }
+            if (st == 0 && steps == 3) {  // statistics of half 0 only; its output comes in step 2
+#pragma unroll
+                for (int q = 0; q < 2; ++q) mean0[q] = mh[q], m2_0[q] = m2h[q];
+                continue;
+            }
+            if (st < 2) {
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    if (steps == 1) {
+                        mean[q] = mh[q];
+                        rstd[q] = rsqrtf(m2h[q] * inv_half + p.eps);
+                    } else {
+                        // two equal halves: M2 = M2_0 + M2_1 + n_half ((mean_0 - mean)^2 + (mean_1 - mean)^2)
+                        mean[q] = 0.5f * (mean0[q] + mh[q]);
+                        const float d0 = mean0[q] - mean[q], d1 = mh[q] - mean[q];
+                        rstd[q] = rsqrtf((m2_0[q] + m2h[q] + 256.0f * (d0 * d0 + d1 * d1)) * (0.5f * inv_half) + p.eps);
+                    }
+                }
+            }
+            // normalise, activate, store both planes
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                if (rows[q] >= p.M) continue;
+                __nv_bfloat16* ohi = p.out_hi + (long long)rows[q] * p.ldo_s + c0 + cq;
+                __nv_bfloat16* olo = ohi + p.out_plane;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const int col = c0 + 8 * j + cq;
+                    const float2 ga = *reinterpret_cast<const float2*>(p.gamma + col);
+                    const float2 be = *reinterpret_cast<const float2*>(p.beta + col);
+                    const float y0 = apply_act(fmaf((acc[4 * j + 2 * q] - mean[q]) * rstd[q], ga.x, be.x), p.act);
+                    const float y1 = apply_act(fmaf((acc[4 * j + 2 * q + 1] - mean[q]) * rstd[q], ga.y, be.y), p.act);
+                    __nv_bfloat16 h0, l0, h1, l1;
                     split_bf16(y0, h0, l0);
                     split_bf16(y1, h1, l1);
-                    split_bf16(y2, h2, l2);
-                    split_bf16(y3, h3, l3);
-                    hh[t >> 1] = pack_bf16x2(h0, h1), hh[(t >> 1) + 1] = pack_bf16x2(h2, h3);
-                    ll[t >> 1] = pack_bf16x2(l0, l1), ll[(t >> 1) + 1] = pack_bf16x2(l2, l3);
-                }
-                if (row_ok) {
-#pragma unroll
-                    for (int q4 = 0; q4 < 4; ++q4) {
-                        *reinterpret_cast<uint4*>(ohi + col0 + q4 * 8) = make_uint4(hh[q4 * 4], hh[q4 * 4 + 1], hh[q4 * 4 + 2], hh[q4 * 4 + 3]);
-                        *reinterpret_cast<uint4*>(olo + col0 + q4 * 8) = make_uint4(ll[q4 * 4], ll[q4 * 4 + 1], ll[q4 * 4 + 2], ll[q4 * 4 + 3]);
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&acc_empty));
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// 2-CTA variant (tcgen05 cta_group::2): two CTAs of a cluster (consecutive m-tiles) act as one 256 x BN MMA.
-// Each CTA streams its own 128 A rows and only HALF of the W tile (BN/2 rows); the tensor cores of the pair read
-// both halves, so the operand bytes ingested per SM and flop drop by 1/3 (BN=256: 64 KB instead of 96 KB per
-// 64-deep k-block) - the quantity that bounds this GEMM (profiles/r01_gemm_qkv_ncu_full.md).
-//   * TMEM is allocated/deallocated by warp 1 of BOTH CTAs with cta_group::2,
-//   * both producers signal the LEADER's full barrier (cp.async.bulk.tensor ... cta_group::2),
-//   * only the leader issues tcgen05.mma.cta_group::2; its commits are multicast to both CTAs' barriers,
-//   * each CTA runs the shared epilogue on its own 128 accumulator rows.
-// ---------------------------------------------------------------------------------------------
-template <int MAXBN, int STAGES>
-struct Gemm2Smem {
-    static constexpr int A_TILE = GEMM_BM * GEMM_BK * 2;
-    static constexpr int BH_TILE = (MAXBN / 2) * GEMM_BK * 2;  // this CTA's half of the W tile, one plane
-    static constexpr int STAGE = 2 * A_TILE + 2 * BH_TILE;
-    static constexpr int TOTAL = STAGES * STAGE + 1024;
-    static constexpr int TMEM_COLS = MAXBN <= 64 ? 64 : (MAXBN <= 128 ? 128 : 256);
-};
-
-__device__ __forceinline__ void tma_load_5d_2sm(uint32_t smem_dst, const void* tmap, uint32_t leader_bar, int c0, int c1, int c2,
-                                                int c3, int c4) {
-    asm volatile(
-        "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_dst), "l"(tmap), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-        : "memory");
-}
-
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {  // arrives on `bar` in both CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-
-template <int MAXBN, int STAGES>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_bh, const GemmShape shape,
-                const GemmEpilogue ep) {
-    pdl_launch_dependents();
-    using S = Gemm2Smem<MAXBN, STAGES>;
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t full_bar[STAGES];   // used in the leader CTA only
-    __shared__ __align__(8) uint64_t empty_bar[STAGES];
-    __shared__ __align__(8) uint64_t tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
-
-    const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-    unsigned char* smem_aligned = smem_dyn + (smem_base - smem_u32(smem_dyn));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m_tile = blockIdx.x, n_tile = blockIdx.y;  // the CTA pair must be adjacent in the cluster x dimension
-    const int z = blockIdx.z;
-    const int split = z % shape.split_k;
-    const int bz = z / shape.split_k;
-    const int b1 = bz % shape.nb1, b2 = bz / shape.nb1;
-    const int BN = shape.bn, BNH = shape.bn / 2;
-    const uint32_t crank = cluster_ctarank();  // 0 = leader of the pair
-    const bool leader = crank == 0;
-
-    const int kb_total = (shape.K + GEMM_BK - 1) / GEMM_BK;
-    const int kb_per = (kb_total + shape.split_k - 1) / shape.split_k;
-    const int kb_begin = split * kb_per;
-    const int kb_end = min(kb_total, kb_begin + kb_per);
-    const int num_kb = max(0, kb_end - kb_begin);
-    const bool lo_pass = shape.passes == 3;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmap_a);
-        tma_prefetch_desc(&tmap_bh);
-        for (int s = 0; s < STAGES; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 1);
-        }
-        mbar_init(smem_u32(&tmem_full_bar), 1);
-        fence_mbar_init();
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)), "r"((uint32_t)S::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = tmem_base_smem;
-    cluster_sync_all();  // both CTAs' barriers and TMEM are ready before any cross-CTA signal
-    pdl_wait();
-
-    if (warp == 0) {
-        // ===================== TMA producers (both CTAs) =====================
-        if (lane < 2) {
-            const uint32_t cta_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(S::A_TILE + BNH * GEMM_BK * 2);
-            for (int i = 0; i < num_kb; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-                mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1u);
-                const uint32_t fb_leader = mapa_shared(smem_u32(&full_bar[s]), 0);  // the leader's barrier collects both CTAs' bytes
-                const uint32_t sa = smem_base + s * S::STAGE;
-                const int k0 = (kb_begin + i) * GEMM_BK;
-                if (lane == 0) {
-                    if (leader) mbar_arrive_expect_tx(smem_u32(&full_bar[s]), 2u * cta_bytes);
-                    tma_load_5d_2sm(sa, &tmap_a, fb_leader, k0, m_tile * GEMM_BM, 0, b1, b2);
-                } else {
-                    tma_load_5d_2sm(sa + 2 * S::A_TILE, &tmap_bh, fb_leader, k0, n_tile * BN + (int)crank * BNH, 0, b1, b2);
+                    *reinterpret_cast<uint32_t*>(ohi + 8 * j) = pack_bf16x2(h0, h1);
+                    *reinterpret_cast<uint32_t*>(olo + 8 * j) = pack_bf16x2(l0, l1);
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (leader) {
-            const uint32_t idesc = umma_idesc_bf16(2 * GEMM_BM, BN);
-            for (int i = 0; i < num_kb; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-                mbar_wait(smem_u32(&full_bar[s]), ph);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t sa = smem_base + s * S::STAGE;
-                    const uint64_t a_hi = umma_desc_k_sw128(sa);
-                    const uint64_t a_lo = umma_desc_k_sw128(sa + S::A_TILE);
-                    const uint64_t b_hi = umma_desc_k_sw128(sa + 2 * S::A_TILE);
-                    const uint64_t b_lo = umma_desc_k_sw128(sa + 2 * S::A_TILE + BNH * GEMM_BK * 2);
-#pragma unroll
-                    for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16_2sm(tmem_base, a_hi + 2 * k, b_hi + 2 * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    if (lo_pass) {
-#pragma unroll
-                        for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16_2sm(tmem_base, a_lo + 2 * k, b_hi + 2 * k, idesc, 1u);
-#pragma unroll
-                        for (int k = 0; k < GEMM_BK / 16; ++k) umma_bf16_2sm(tmem_base, a_hi + 2 * k, b_lo + 2 * k, idesc, 1u);
-                    }
-                    umma_commit_2sm(smem_u32(&empty_bar[s]));
-                    if (i == num_kb - 1) umma_commit_2sm(smem_u32(&tmem_full_bar));
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        gemm_epilogue(shape, ep, smem_aligned, tmem_base, smem_u32(&tmem_full_bar), warp, lane, m_tile, n_tile, b1, b2, split, num_kb, BN);
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)S::TMEM_COLS) : "memory");
     }
 }
 
@@ -1261,7 +717,7 @@ static PFN_encodeTiled get_encode() {
     return fn;
 }
 
-static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes = 1, int bk = GEMM_BK) {
+static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes = 1) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) return PSAM_ERR_UNSUPPORTED;
     const int nb1 = op->nb1 > 0 ? op->nb1 : 1, nb2 = op->nb2 > 0 ? op->nb2 : 1;
@@ -1273,10 +729,10 @@ static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_ro
     for (int i = 0; i < 4; ++i)
         if (strides[i] % 16) return PSAM_ERR_ARG;
     if (((uintptr_t)op->hi) % 16) return PSAM_ERR_ARG;
-    cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1, 1};
+    cuuint32_t box[5] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1, 1};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(op->hi), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? PSAM_OK : (int)(1000 + r);
 }
@@ -1285,95 +741,29 @@ int make_operand_map_ext(CUtensorMap* map, const psam_operand* op, int box_rows,
     return make_operand_map(map, op, box_rows, box_planes);
 }
 
-template <int MAXBN, int STAGES, int BK = 64, int EPQ = GEMM_EPI_PER_QUARTER, int RES = 1>
-static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& mbmc, const GemmShape& sh,
-                       const GemmEpilogue& ep, cudaStream_t stream) {
-    auto kern = gemm_tc_kernel<MAXBN, STAGES, BK, EPQ, RES>;
-    using S = GemmSmem<MAXBN, STAGES, BK>;
+template <int BN, int STAGES>
+static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmShape& sh, const GemmEpilogue& ep, cudaStream_t stream) {
+    auto kern = gemm_wgmma_kernel<BN, STAGES>;
+    using S = GemmSmem<BN, STAGES>;
     PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    const int mt = ceil_div(ceil_div(sh.M, GEMM_BM), sh.cm) * sh.cm;  // pad the m-tiles to whole clusters
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)ceil_div(sh.N, sh.bn), (unsigned)mt, (unsigned)(sh.nb1 * sh.nb2 * sh.split_k));
-    cfg.blockDim = dim3(gemm_threads(EPQ));
-    cfg.dynamicSmemBytes = S::TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    int na = 0;
-    if (sh.cm > 1) {
-        attr[na].id = cudaLaunchAttributeClusterDimension;
-        attr[na].val.clusterDim.x = 1;
-        attr[na].val.clusterDim.y = (unsigned)sh.cm;
-        attr[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    if (pdl_enabled()) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    PSAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mb, mbmc, sh, ep));
+    const dim3 grid((unsigned)ceil_div(sh.N, BN), (unsigned)ceil_div(sh.M, GEMM_BM), (unsigned)(sh.nb1 * sh.nb2 * sh.split_k));
+    PSAM_CUDA_TRY(psam::launch(kern, grid, dim3(GEMM_THREADS), (size_t)S::TOTAL, stream, ma, mb, sh, ep));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }
 
-template <int MAXBN, int STAGES, int BK, int EPQ>
-static int launch_gemm_persist(const CUtensorMap& ma, const CUtensorMap& mb, const GemmShape& sh, const GemmEpilogue& ep,
-                               int ctas, cudaStream_t stream) {
-    auto kern = gemm_tc_persist_kernel<MAXBN, STAGES, BK, EPQ>;
-    using S = GemmSmem<MAXBN, STAGES, BK>;
-    constexpr int SMEM = STAGES * S::STAGE + 4 * EPQ * 32 * EPI_PITCH * 4 + 1024;
-    static_assert(SMEM <= 232448, "shared memory budget of one SM");
-    PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    PSAM_CUDA_TRY(psam::launch(kern, dim3((unsigned)ctas), dim3(gemm_threads(EPQ)), (size_t)SMEM, stream, ma, mb, sh, ep));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
-}
-
-template <int MAXBN, int STAGES>
-static int launch_gemm2(const CUtensorMap& ma, const CUtensorMap& mbh, const GemmShape& sh, const GemmEpilogue& ep,
-                        cudaStream_t stream) {
-    auto kern = gemm_tc2_kernel<MAXBN, STAGES>;
-    using S = Gemm2Smem<MAXBN, STAGES>;
-    PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    const int mt = ceil_div(ceil_div(sh.M, GEMM_BM), 2) * 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)mt, (unsigned)ceil_div(sh.N, sh.bn), (unsigned)(sh.nb1 * sh.nb2 * sh.split_k));
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = S::TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;  // cta_group::2 pairs are the CTAs with consecutive ranks along x
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    int na = 1;
-    if (pdl_enabled()) {
-        attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attr[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = na;
-    PSAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mbh, sh, ep));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
-}
-
-// Output-tile width: multiple of 32 in [32, 256] minimising (waves over 148 SMs) x (per-CTA cost), where the
-// per-CTA cost follows the operand bytes streamed per k-block (the kernel is L2->SM bandwidth bound).
+// Output-tile width: 64, 128 or 256 minimising (waves over the 132 SMs of an H100) x (per-CTA cost), where the per-CTA cost
+// follows the operand bytes streamed per k-block.  The throughput policy (several clouds in flight share the SMs) minimises
+// the total SM-time instead, which favours wide tiles (fewer operand bytes per flop).
 static int choose_bn(int M, int N, int K, int batches, int split_k, bool throughput) {
     const int mt = ceil_div(M, GEMM_BM);
     const int kb = ceil_div(ceil_div(K, GEMM_BK), split_k);
     int best = 128;
     double best_cost = 1e30;
-    for (int bn = (N >= 64 ? 64 : 32); bn <= 256; bn += 32) {
-        if (bn > 32 && bn - 32 >= N) break;
+    for (int bn = 64; bn <= 256; bn *= 2) {
+        if (bn > 64 && bn / 2 >= N) break;
         const long long tiles = (long long)ceil_div(N, bn) * mt * batches * split_k;
-        const long long waves = (tiles + 147) / 148;
-        // latency policy: waves x per-CTA time; throughput policy (several clouds in flight share the SMs):
-        // total SM-time = tiles x per-CTA time, which favours wide tiles (fewer operand bytes per flop)
+        const long long waves = (tiles + 131) / 132;
         const double per_cta = 6.0 * 256 + (double)kb * (128 + bn) + 0.35 * bn * 4;
         const double cost = throughput ? (double)tiles * per_cta : (double)waves * per_cta;
         if (cost < best_cost - 1e-9) best_cost = cost, best = bn;
@@ -1400,7 +790,6 @@ extern "C" int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, co
     sh.split_k = split_k;
     sh.passes = passes;
     const int variant = o->variant;
-    sh.prefetch = (variant >> 12) & 15;  // k-blocks of W to prefetch into L2 ahead of the TMA loads
     GemmEpilogue ep;
     ep.out_f32 = o->out_f32, ep.ldo = o->ldo, ep.out_b1 = o->out_b1, ep.out_b2 = o->out_b2;
     ep.out_hi = (__nv_bfloat16*)o->out_hi, ep.out_plane = o->out_plane, ep.ldo_s = o->ldo_s;
@@ -1438,101 +827,16 @@ extern "C" int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, co
     if (ep.gmax && (ep.group_rows <= 0 || ep.group_rows % 32 || ep.accumulate || ep.resid || ep.act || ep.swiglu || sh.nb1 * sh.nb2 != 1)) return PSAM_ERR_ARG;
     if (ep.swiglu && ((!ep.out_hi == !ep.out_f32) || ep.accumulate || ep.resid || ep.act || (sh.N & 1))) return PSAM_ERR_ARG;
     int bn = choose_bn(sh.M, sh.N, sh.K, sh.nb1 * sh.nb2, sh.split_k, o->tile_hint == 1);
-    if (o->tile_hint >= 32 && o->tile_hint <= 256 && o->tile_hint % 32 == 0) bn = o->tile_hint;
+    if (o->tile_hint >= 32 && o->tile_hint <= 256 && o->tile_hint % 32 == 0) bn = o->tile_hint <= 64 ? 64 : (o->tile_hint <= 128 ? 128 : 256);
     sh.bn = bn;
-    const int mtiles = ceil_div(sh.M, GEMM_BM);
-    // 2-CTA path (cta_group::2): pairs of m-tiles, each CTA streams half of the W tile.  Opt-in: variant bit 0x1.
-    {
-        // Throughput policy with many rows (>= 16 m-tiles: several clouds per request) and deep K: the pair halves the W bytes
-        // each SM ingests.  MEASURED round 2: c3 (4 clouds per graph, M = 2048) 444 -> 474 clouds/s; c2 (M = 512) 694 -> 682, so
-        // single-cloud requests keep the 1-CTA kernel.  Launches with >= 2 tiles per SM go to the persistent kernel below.
-        const long long tiles256 = (long long)ceil_div(sh.N, 256) * mtiles * sh.nb1 * sh.nb2 * sh.split_k;
-        const bool auto2 = o->tile_hint == 1 && mtiles >= 16 && sh.K >= 1024 && sh.N >= 256 && tiles256 < 2 * 148 &&
-                           !(variant & (GV_PERSIST | GV_DUAL | GV_BK32 | GV_NO_DUAL)) && ((variant >> 8) & 15) == 0;
-        const int use2 = (variant & GV_2CTA) || auto2;
-        if (use2 && mtiles >= 2 && sh.N >= 128) {
-            int bn2 = (o->tile_hint == 1 || sh.N >= 256) ? 256 : 128;
-            if (o->tile_hint >= 64 && o->tile_hint <= 256 && o->tile_hint % 64 == 0) bn2 = o->tile_hint;
-            if (bn2 > 128 && (long long)ceil_div(sh.N, 256) * ceil_div(mtiles, 2) * sh.nb1 * sh.nb2 * sh.split_k * 2 < 100 && o->tile_hint != 1) bn2 = 128;
-            sh.bn = bn2;
-            sh.cm = 2;
-            CUtensorMap ma2, mbh;
-            int rc2 = make_operand_map(&ma2, a, GEMM_BM, passes == 3 ? 2 : 1);
-            if (rc2) return rc2;
-            rc2 = make_operand_map(&mbh, w, bn2 / 2, passes == 3 ? 2 : 1);
-            if (rc2) return rc2;
-            return bn2 <= 128 ? launch_gemm2<128, 4>(ma2, mbh, sh, ep, stream) : launch_gemm2<256, 3>(ma2, mbh, sh, ep, stream);
-        }
-    }
-    // CTAs of consecutive m-tiles form a cluster and share each W tile through TMA multicast
-    // MEASURED (B200, config c2, 8 clouds in flight): cluster 4 -> 581 clouds/s, no cluster -> 626 clouds/s: the L2
-    // already merges the concurrent requests of the 4 m-tile CTAs for the same W lines, and the cluster couples their
-    // progress.  Multicast therefore stays opt-in (variant bits 8-11 = cluster size 2|4).
-    int cm = 1;
-    {
-        const int v = (variant >> 8) & 15;
-        const int cap = mtiles >= 4 ? 4 : (mtiles >= 2 ? 2 : 1);
-        if (v == 1 || v == 2 || v == 4) cm = v < cap ? v : cap;
-    }
-    while (cm > 1 && (bn / cm) % 8) cm /= 2;
-    sh.cm = cm;
-    CUtensorMap ma, mb, mbmc;
+    CUtensorMap ma, mb;
     int rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1);
     if (rc) return rc;
     rc = make_operand_map(&mb, w, bn, passes == 3 ? 2 : 1);
     if (rc) return rc;
-    rc = make_operand_map(&mbmc, w, bn / cm, 1);
-    if (rc) return rc;
-    // Persistent kernel (double-buffered TMEM accumulator, stage ring running across tiles): whenever a CTA would get at
-    // least two tiles (many-row GEMMs: the mini-PointNet, batched clouds), or on request (GV_PERSIST; bits 16-19 = tiles per
-    // CTA to aim for, which trades SMs occupied by this launch against its length).
-    {
-        int nsm = 148, devid = 0;
-        if (cudaGetDevice(&devid) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, devid);
-        const long long total = (long long)ceil_div(sh.N, bn) * mtiles * sh.nb1 * sh.nb2 * sh.split_k;
-        const int want = (variant >> 16) & 15;
-        const bool persist = cm == 1 && !(variant & GV_NO_PERSIST) && total < (1ll << 30) &&
-                             ((variant & GV_PERSIST) || total >= 2ll * nsm);
-        if (persist) {
-            long long per = ceil_div_ll(total, nsm);       // tiles per CTA when the launch spreads over all SMs
-            if (want > per) per = want;
-            const int ctas = (int)ceil_div_ll(total, per);  // balanced: every CTA gets `per` (or per - 1) tiles
-            const int bkp = bn > 128 ? 32 : 64;
-            rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1, bkp);
-            if (rc) return rc;
-            rc = make_operand_map(&mb, w, bn, passes == 3 ? 2 : 1, bkp);
-            if (rc) return rc;
-            // short main loops (the mini-PointNet: K = 128 ... 512) are bounded by the epilogue: eight epilogue warps and
-            // three stages; long ones by operand latency: four stages, four epilogue warps
-            if (bn > 128 && sh.K <= 512) return launch_gemm_persist<256, 3, 32, 2>(ma, mb, sh, ep, ctas, stream);
-            if (bn > 128) return launch_gemm_persist<256, 4, 32, 1>(ma, mb, sh, ep, ctas, stream);
-            if (bn > 64) return launch_gemm_persist<128, 3, 64, 1>(ma, mb, sh, ep, ctas, stream);
-            return launch_gemm_persist<64, 4, 64, 1>(ma, mb, sh, ep, ctas, stream);
-        }
-    }
-    // wide tiles: the dual-resident configuration (two 97 KB CTAs per SM, BK = 32, 2 stages each) on request (GV_DUAL).
-    // GV_BK32: one CTA per SM with 4 half-size stages.  MEASURED round 1: 611 vs 618 clouds/s - no gain, opt-in.
-    // MEASURED round 2 (c2, 8 clouds in flight, 3 repeats): dual-resident 606 / 644 clouds/s (LN-free / LayerNorm blocks) vs
-    // 642 / 635 for the one-CTA-per-SM kernel, and +1.8 ms single-stream latency: with two 2-stage CTAs per SM neither can hide
-    // the operand latency alone while the other is in its prologue / epilogue.  Opt-in (GV_DUAL) only.
-    const bool dual = bn > 160 && cm == 1 && (variant & GV_DUAL) && !(variant & GV_NO_DUAL);
-    if (bn > 160 && cm == 1 && (dual || (variant & GV_BK32))) {
-        rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1, 32);
-        if (rc) return rc;
-        rc = make_operand_map(&mb, w, bn, passes == 3 ? 2 : 1, 32);
-        if (rc) return rc;
-        if (dual) return launch_gemm<256, 2, 32, 2, 2>(ma, mb, mb, sh, ep, stream);
-        return launch_gemm<256, 4, 32>(ma, mb, mb, sh, ep, stream);
-    }
-    if (bn <= 64) return launch_gemm<64, 4>(ma, mb, mbmc, sh, ep, stream);
-    if (bn <= 128) return launch_gemm<128, 3>(ma, mb, mbmc, sh, ep, stream);
-    if (bn <= 160) return launch_gemm<160, 3>(ma, mb, mbmc, sh, ep, stream);
-    // GV_TWO_ISSUERS: two MMA-issuing warps per wide one-shot tile.  MEASURED round 2: the issue-rate probe promised 171 -> 151
-    // clk per 128 x 256 x 16 MMA, but the kernel gains nothing in isolation (qkv 1256 vs 1266, fc1 1197 vs 1238 TFLOP/s at 8 streams)
-    // and loses in the step (616 vs 672 clouds/s, twelve epilogue warps instead of sixteen): the two-stage main loop is bound by
-    // operand latency, not by issue.  Opt-in.
-    if (cm == 1 && (variant & GV_TWO_ISSUERS) && sh.prefetch == 0) return launch_gemm_duo<256, 2>(ma, mb, sh, ep, stream);
-    return launch_gemm<256, 2>(ma, mb, mbmc, sh, ep, stream);
+    if (bn == 64) return launch_gemm<64, 4>(ma, mb, sh, ep, stream);
+    if (bn == 128) return launch_gemm<128, 3>(ma, mb, sh, ep, stream);
+    return launch_gemm<256, 2>(ma, mb, sh, ep, stream);
 }
 
 extern "C" int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand* w, const float* gbias, long long ld_gbias, int group_rows,
@@ -1556,13 +860,13 @@ extern "C" int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand*
     if (rc) return rc;
     rc = make_operand_map(&mw, w, 256, passes == 3 ? 2 : 1);
     if (rc) return rc;
-    int nsm = 148, devid = 0;
+    int nsm = 132, devid = 0;
     if (cudaGetDevice(&devid) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, devid);
     const int mt = ceil_div(p.M, GEMM_BM);
     const int per = ceil_div(mt, nsm);
     const int ctas = ceil_div(mt, per);
     PSAM_CUDA_TRY(cudaFuncSetAttribute(gemm_rowln_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RL_SMEM));
-    PSAM_CUDA_TRY(psam::launch(gemm_rowln_kernel, dim3((unsigned)ctas), dim3(RL_THREADS), (size_t)RL_SMEM, stream, ma, mw, p));
+    PSAM_CUDA_TRY(psam::launch(gemm_rowln_kernel, dim3((unsigned)ctas), dim3(GEMM_THREADS), (size_t)RL_SMEM, stream, ma, mw, p));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }

@@ -1,4 +1,4 @@
-// kNN grouping and 3-NN interpolation weights for sm_100a.
+// kNN grouping and 3-NN interpolation weights for sm_90a.
 //
 // Replaces pc_sam/model/common.py: knn_points (:27-56, torch.cdist + torch.topk), the gathers of
 // KNNGrouper.forward / group_with_centers_and_knn (:99-123, :126-187) and compute_interp_weights
@@ -469,7 +469,7 @@ __global__ void group_gather_kernel(const float* __restrict__ xyz, const float* 
 // 3 nearest centres per point + inverse-squared-distance weights (common.py:238-255).
 // FOUR lanes per point: lane `part` scans the centres part, part + 4, ... keeping its three nearest, then two shuffle
 // rounds merge the four sorted triples (order: distance, then centre index - what the ascending scan with a strict '<'
-// produces).  One thread per point left 32768 / 32 = 1024 warps for 148 SMs (two per scheduler, a 512-long dependent
+// produces).  One thread per point left 32768 / 32 = 1024 warps for 132 SMs (two per scheduler, a 512-long dependent
 // chain each: 28 us); a quarter of the chain on four times the warps.
 struct Near3 {
     float d0, d1, d2;
@@ -809,7 +809,7 @@ extern "C" int psam_group_gather_f32(const float* xyz, const float* feats, const
     using namespace psam;
     if (!xyz || !feats || !centers || !knn_idx || !groups_out || B <= 0 || rep <= 0 || C < 0) return PSAM_ERR_ARG;
     const long long total = (long long)B * rep * G * K;
-    const int blocks = (int)min((long long)148 * 16, ceil_div_ll(total, 256));
+    const int blocks = (int)min((long long)132 * 16, ceil_div_ll(total, 256));
     PSAM_CUDA_TRY(psam::launch(group_gather_kernel, dim3(blocks), dim3(256), (size_t)(0), stream, xyz, feats, centers, knn_idx, center_idx, B * rep, rep, N, G, K, C,
                                                     radius > 0.f ? 1.0f / radius : 1.0f, groups_out));
     PSAM_LAUNCH_CHECK();

@@ -1,4 +1,4 @@
-"""Evaluation driver with the behaviour of /root/reference/evaluation/eval_kitti.py:284-398 on top of the sm_100a
+"""Evaluation driver with the behaviour of the reference's evaluation/eval_kitti.py:284-398 on top of the sm_90a
 path: binary PLY crops (fields x y z R G B label) -> normalisation -> per-cloud group-count / group-size override ->
 ``model(**data, is_eval=True)`` (iterative GT-driven prompting) -> IoU per prompt iteration, averaged per object class
 and overall.  The dataset glob is an argument instead of a hard-coded path; every crop is rotated by the reference's
@@ -82,7 +82,7 @@ def evaluate(model, files: Sequence[str], rotation: Optional[np.ndarray] = None,
     """Returns {"total": [prompt_iters], "per_object": {name: [prompt_iters]}, "object_mean": [prompt_iters]}.
 
     Crops are independent, so with several processes (one per GPU, torch.distributed initialised) each rank evaluates a
-    contiguous slice of `files` and the per-crop IoU rows are all-gathered once at the end (SURVEY.md 8e); every rank
+    contiguous slice of `files` and the per-crop IoU rows are all-gathered once at the end; every rank
     returns the same aggregate.  Single process: rank/world default to 0/1."""
     import torch.distributed as dist
 

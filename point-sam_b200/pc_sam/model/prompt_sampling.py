@@ -1,6 +1,6 @@
 """Ground-truth-driven prompt sampling for PointCloudSAM.forward(is_eval=True)
 (/root/reference/pc_sam/model/common.py:287-474: sample_prompts_adapter, sample_fixed_points,
-sample_furthest_points_from_border).  SURVEY.md section 8(f) rank 1 ("next" row).
+sample_furthest_points_from_border).  
 
 The reference walks (cloud, mask) pairs in Python, compacts foreground/background points, calls torkit3d's chamfer
 kernel per region and compares the results on the host.  Here every (cloud, mask, region) is evaluated by one

@@ -1,4 +1,4 @@
-"""Build libpsam_b200.so (CUDA kernels + C ABI) in-tree for sm_100a with nvcc."""
+"""Build libpsam_b200.so (CUDA kernels + C ABI) in-tree for sm_90a (H100) with nvcc."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIBDIR = os.path.join(PKG, "lib")
 LIB = os.path.join(LIBDIR, "libpsam_b200.so")
 SOURCES = ["fps.cu", "knn.cu", "gemm_tc.cu", "attention_tc.cu", "elementwise.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -39,7 +39,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
     if force or not _newer(LIB, objs):
-        subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+        subprocess.check_call(["nvcc", "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

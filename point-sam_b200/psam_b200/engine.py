@@ -25,22 +25,21 @@ FUSED_ATTENTION_LONG = os.environ.get("PSAM_FUSED_ATTENTION_LONG", "1") != "0"
 ATTENTION_TWOPASS = os.environ.get("PSAM_ATTENTION_TWOPASS", "0") == "1"  # A/B: first-generation two-pass kernels
 FUSED_INNER_LN = os.environ.get("PSAM_FUSED_INNER_LN", "1") != "0"  # SwiGLU.norm folded into the fc1 / fc2 GEMM epilogues
 FUSED_MASK_DOT = os.environ.get("PSAM_FUSED_MASK_DOT", "1") != "0"
-# the decoder's projections of the G patch rows (keys of the two-way transformer, 512 rows at c2) on the tcgen05 GEMM instead of
+# the decoder's projections of the G patch rows (keys of the two-way transformer, 512 rows at c2) on the tensor-core GEMM instead of
 # the fp32 SIMT linear; the token-side (<= 16 rows) projections stay SIMT
 DECODER_TC = os.environ.get("PSAM_DECODER_TC", "1") != "0"
 # norm1 / norm2 / fc_norm folded into the qkv / fc1 / out_proj GEMMs: the producer of the residual stream (pos_embed, proj and
 # fc2 GEMM epilogues) writes x as fp32 + split-bf16 and accumulates the row statistics, so no LayerNorm kernel runs in a block
 # EVA-giant heads (dh = 88) on the fused attention kernel (64 + 24 columns, zero padded by TMA).  Full-size parity of the 40-block
-# model holds with it (tests/test_gpu_model.py::test_config5_full_size_vs_fp32_oracle_on_gpu, both LayerNorm forms); c5: 213 -> 243
-# clouds/s (profiles/r02_bench_c5_fused_dh88.json).  PSAM_FUSED_ATTENTION_DH88=0 selects the unfused tensor-core path (QK^T GEMM,
+# model holds with it (tests/test_gpu_model.py::test_config5_full_size_vs_fp32_oracle_on_gpu, both LayerNorm forms).
+# PSAM_FUSED_ATTENTION_DH88=0 selects the unfused tensor-core path (QK^T GEMM,
 # softmax, V transpose, PV GEMM) it replaces.
 FUSED_ATTENTION_DH88 = os.environ.get("PSAM_FUSED_ATTENTION_DH88", "1") != "0"
 FUSED_ROW_LN = os.environ.get("PSAM_FUSED_ROW_LN", "1") != "0"  # mini-PointNet conv2[0] + LayerNorm + GELU in one row-complete GEMM
 FUSED_BLOCK_LN = os.environ.get("PSAM_FUSED_BLOCK_LN", "1") != "0"  # capability: pack the LayerNorm-folded weights as well
 # When the LayerNorm-free form of the ViT blocks is USED (both weight sets are packed):
-#   "auto"   - only inside PipelinedPredictor captures with >= 8 clouds in flight.  MEASURED (c2): at depth 8 the folded form
-#              ties with the LayerNorm kernels (642 vs 645 clouds/s) at 49 fewer launches per cloud; at depth 4 it loses
-#              (543 vs 574) and single-stream latency is 4.0 vs 3.4 ms, because the fold needs split_k = 1 on proj / fc2.
+#   "auto"   - only inside PipelinedPredictor captures with >= 8 clouds in flight: the folded form saves 49 launches per
+#              cloud but needs split_k = 1 on proj / fc2, which costs single-stream latency.
 #   "always" / "never" - forced (tests, experiments; PSAM_BLOCK_LN_POLICY).
 BLOCK_LN_POLICY = os.environ.get("PSAM_BLOCK_LN_POLICY", "auto")
 _fold_ctx = threading.local()
@@ -87,11 +86,11 @@ def _f32(t):
 
 
 def _split_k_for(M: int, N: int, K: int) -> int:
-    """Fill the 148 SMs when the output has few tiles (small-batch inference)."""
+    """Fill the 132 SMs of an H100 when the output has few tiles (small-batch inference)."""
     tiles = ((M + 127) // 128) * ((N + 127) // 128)
     kb = (K + 63) // 64
     s = 1
-    while tiles * s * 2 <= 148 and s * 2 <= max(1, kb // 4):
+    while tiles * s * 2 <= 132 and s * 2 <= max(1, kb // 4):
         s *= 2
     return s
 
@@ -532,8 +531,8 @@ def _run_block(pb: _PackedBlock, x: torch.Tensor, B: int, L: int, D: int, fold=N
         ops.gemm(xn, pb.wqkv, bias=pb.bqkv, out_split=qkv, passes=PASSES)
     att = Split(M, D, dev)
     if FUSED_ATTENTION and (dh == 64 or (dh == 88 and not ATTENTION_TWOPASS and FUSED_ATTENTION_DH88)) and (L <= 512 or FUSED_ATTENTION_LONG):
-        # fused tcgen05 attention: S stays in tensor memory (L <= 512) or streams through a ring of TMEM slots in two
-        # sweeps (longer rows); V^T is read as an MN-major operand
+        # fused wgmma attention: S and P stay in registers, key blocks stream through shared memory; V^T is read as an
+        # MN-major operand
         mk = lambda col: qkv.operand(rows=L, k=dh, col=col, nb1=H, b1_stride=dh, nb2=B, b2_stride=L * qkv.pitch)
         qa, ka, va = mk(0), mk(D), mk(2 * D)
         entry = nv.lib().psam_attention_bf16x3_twopass if ATTENTION_TWOPASS else nv.lib().psam_attention_bf16x3

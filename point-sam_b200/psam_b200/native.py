@@ -113,10 +113,6 @@ def lib():
             fn = getattr(L, name)
             fn.argtypes = args
             fn.restype = c_int
-        # experiment switch behind a debug setter of the library (the library itself reads no environment variable)
-        v = os.environ.get("PSAM_ATTENTION_TILES")
-        if v:
-            L.psam_debug_attention_tiles(int(v))
         _lib = L
     return _lib
 

@@ -1,6 +1,6 @@
 """Data-parallel plumbing: clouds are independent units, so the path shards by contiguous ranges of clouds per
 rank (weights replicated) and needs exactly one collective - the all_gather of per-cloud metrics at the end
-(SURVEY.md section 8e).  Works with any torch.distributed backend (NCCL on the B200 box, gloo in CPU tests)."""
+Works with any torch.distributed backend (NCCL on GPUs, gloo in CPU tests)."""
 from __future__ import annotations
 
 from typing import List, Tuple

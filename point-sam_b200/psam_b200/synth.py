@@ -1,4 +1,4 @@
-"""Deterministic synthetic inputs (SURVEY.md section 8d).  Shared by bench.py, the tests and the golden-vector
+"""Deterministic synthetic inputs.  Shared by bench.py, the tests and the golden-vector
 generator (through oracle/synth.py); pure CPU torch so that every box produces identical tensors."""
 from __future__ import annotations
 

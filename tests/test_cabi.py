@@ -28,7 +28,7 @@ def test_header_symbols_exported(lib_path):
 
     assert sorted(native.EXPORTS) == declared
     lib.psam_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.psam_version()
+    assert b"sm_90a" in lib.psam_version()
 
 
 def test_argument_validation_without_gpu(lib_path):

@@ -1,4 +1,4 @@
-"""CPU tests of the data formats and callers either side of the hot path (SURVEY.md 8(f) rows 2-3): PLY readers,
+"""CPU tests of the data formats and callers either side of the hot path: PLY readers,
 input normalisation, safetensors checkpoints, the hydra-style config instantiation and the demo wire format."""
 import json
 import os

@@ -68,7 +68,7 @@ def test_golden_end_to_end(golden_dir, name, fold_ln, fold_block, monkeypatch):
 
 @pytest.mark.parametrize("tc", [True, False])
 def test_decoder_patch_row_projections_tensor_core_and_simt(tc, monkeypatch):
-    """The two-way transformer's projections of the G patch rows run on the tcgen05 GEMM (keys / keys + pe kept as
+    """The two-way transformer's projections of the G patch rows run on the tensor-core GEMM (keys / keys + pe kept as
     split-bf16 by the LayerNorm that updates them) or on the fp32 SIMT linear: both against the oracle, 2 prompts per
     cloud x 2 masks per cloud (Z = B*M = 4) and a prompt-mask pass."""
     from psam_b200 import engine
@@ -257,7 +257,7 @@ def test_serving_predictors_raise_value_error_for_the_offending_ticket_only():
 
 
 def test_batched_prompt_sampler_vs_reference_fixture_and_oracle(golden_dir):
-    """SURVEY.md 8(f) rank 1: the batched border sampler against the reference's own outputs (fixture) and against the
+    """the batched border sampler against the reference's own outputs (fixture) and against the
     oracle on larger seeded inputs, including the empty-region fallbacks."""
     from pc_sam.model import prompt_sampling as ps
     from psam_b200 import ops
@@ -298,7 +298,7 @@ def test_batched_prompt_sampler_vs_reference_fixture_and_oracle(golden_dir):
 
 
 def test_eval_driver_and_demo_session(tmp_path):
-    """SURVEY.md 8(f) rows 2-3: the evaluation caller (binary PLY -> forward(is_eval=True) -> IoU) and the demo wire
+    """the evaluation caller (binary PLY -> forward(is_eval=True) -> IoU) and the demo wire
     format (ASCII PLY, /segment JSON) on top of the CUDA path, checked against the oracle."""
     import sys
 

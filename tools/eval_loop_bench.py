@@ -1,4 +1,4 @@
-"""Evaluation-loop timing (SURVEY.md 8(d) config c3 shape: 4 clouds per GPU, N=32768, ViT-L, 3 prompt iterations with
+"""Evaluation-loop timing (config c3 shape: 4 clouds per GPU, N=32768, ViT-L, 3 prompt iterations with
 GT-driven prompts; mask encoder active on iterations 2-3): forward(is_eval=True) eager (host checks per iteration)
 vs the same loop replayed as one CUDA graph (PointCloudSAM.make_iterative_predictor).
 usage: python tools/eval_loop_bench.py [--clouds 4] [--masks 1] [--iters 3] [--points 32768] [--steps 20]"""
