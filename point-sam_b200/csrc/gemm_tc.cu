@@ -11,8 +11,13 @@
 // 1e-3 abs / 1e-2 rel parity bound (a single bf16 pass, passes = 1, is ~1e-2 and fails it).
 //
 // Structure (one 128 x BN output tile per CTA, optional split-K over blockIdx.z):
-//   warp 8   : TMA producer - 5-D tensor maps (k, row, plane, batch1, batch2), 128B-swizzled 3-D boxes of
-//              64 bf16 x {128|BN} rows x {hi,lo}, 2-4 stage mbarrier ring
+//   warp 8   : TMA producer - 5-D tensor maps (k, row, plane, batch1, batch2), 3-D boxes of
+//              BK bf16 x {128|BN} rows x {hi,lo} into a ~192 KB mbarrier ring:
+//                BN = 256: BK = 32, 64B swizzle, 4 stages.  With BK = 64 only 2 stages of 96 KB fit, so the TMA of
+//                          k-block i+1 had to land within one k-block of compute, and the main loop ran at about half
+//                          the tensor-core rate; the smaller k-block keeps 2-3 loads in flight while one computes.
+//                BN = 128 / 64: BK = 64, 128B swizzle, 3 / 4 stages (measured on H100: BK = 32 with 6 / 8 stages was
+//                          slower at these widths).
 //   warps 0-7: two consumer warpgroups (rows 0-63 / 64-127 of the tile), wgmma m64nBNk16 from shared memory
 //              into fp32 registers; one wgmma group stays in flight while the previous stage is released.
 //              Epilogue: the accumulators are staged as an fp32 tile in the (then idle) stage memory, and each
@@ -29,9 +34,9 @@
 namespace psam {
 
 constexpr int GEMM_BM = 128;
-constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 288;  // two consumer warpgroups + one TMA warp
-constexpr int GEMM_A_TILE = GEMM_BM * GEMM_BK * 2;  // bytes per plane of an A stage
+constexpr int GEMM_THREADS = 288;     // two consumer warpgroups + one TMA warp
+constexpr int GEMM_RING = 192 * 1024;  // shared memory of the operand ring
+__host__ __device__ constexpr int gemm_bk(int bn) { return bn == 256 ? 32 : 64; }  // k-block of a tile width
 // psam_gemm_out.variant bits.  GV_SCALAR_EPI forces the scalar epilogue; the other bits select kernels of other
 // architectures and are accepted without effect, so callers built for them keep working.
 constexpr int GV_SCALAR_EPI = 0x4;
@@ -69,10 +74,13 @@ struct GemmShape {
     int bn;      // output-tile width (64, 128 or 256)
 };
 
-template <int BN, int STAGES>
+template <int BN>
 struct GemmSmem {
-    static constexpr int B_TILE = BN * GEMM_BK * 2;  // bytes per plane
-    static constexpr int STAGE = 2 * GEMM_A_TILE + 2 * B_TILE;
+    static constexpr int BK = gemm_bk(BN);
+    static constexpr int A_TILE = GEMM_BM * BK * 2;  // bytes per plane
+    static constexpr int B_TILE = BN * BK * 2;
+    static constexpr int STAGE = 2 * A_TILE + 2 * B_TILE;
+    static constexpr int STAGES = GEMM_RING / STAGE;  // 4 at BN = 256, 3 at BN = 128, 4 at BN = 64
     static constexpr int PITCH = BN + 4;              // floats per row of the staged output tile
     static constexpr int EPI = GEMM_BM * PITCH * 4;   // the staged tile reuses the stage memory
     static constexpr int TOTAL = (STAGES * STAGE > EPI ? STAGES * STAGE : EPI) + 1024;  // + alignment slack
@@ -399,19 +407,22 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
 // Named barrier of the 256 consumer threads (the TMA warp does not take part).
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// One k-block of the split-bf16 product into the warpgroup's 64 x BN accumulator: 4 k-steps per pass.
-template <int BN>
+// One k-block of the split-bf16 product into the warpgroup's 64 x BN accumulator: BK / 16 k-steps per pass.  Tiles of
+// BK = 64 are 128B-swizzled, tiles of BK = 32 64B-swizzled (rows of 128 / 64 bytes, as the TMA boxes lay them out).
+template <int BN, int BK>
 __device__ __forceinline__ void gemm_kblock(float (&acc)[BN / 2], uint32_t a_hi_addr, uint32_t a_lo_addr, uint32_t b_hi_addr,
                                             uint32_t b_lo_addr, bool lo_pass) {
-    const uint64_t a_hi = gmma_desc_k(a_hi_addr), b_hi = gmma_desc_k(b_hi_addr);
+    static_assert(BK == 32 || BK == 64, "k-block of 32 or 64");
+    auto desc = [](uint32_t addr) { return BK == 64 ? gmma_desc_k(addr) : gmma_desc_k_sw64(addr); };
+    const uint64_t a_hi = desc(a_hi_addr), b_hi = desc(b_hi_addr);
 #pragma unroll
-    for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
+    for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_hi + 2 * k, 1u);
     if (lo_pass) {
-        const uint64_t a_lo = gmma_desc_k(a_lo_addr), b_lo = gmma_desc_k(b_lo_addr);
+        const uint64_t a_lo = desc(a_lo_addr), b_lo = desc(b_lo_addr);
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+        for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
+        for (int k = 0; k < BK / 16; ++k) wgmma_ss<BN>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
     }
 }
 
@@ -427,12 +438,13 @@ __device__ __forceinline__ void stage_acc(float* tile, int pitch, int row_base, 
     }
 }
 
-template <int BN, int STAGES>
+template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmShape shape,
                   const GemmEpilogue ep) {
     pdl_launch_dependents();
-    using S = GemmSmem<BN, STAGES>;
+    using S = GemmSmem<BN>;
+    constexpr int STAGES = S::STAGES;
     extern __shared__ unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[STAGES];
     __shared__ __align__(8) uint64_t empty_bar[STAGES];
@@ -446,7 +458,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int bz = z / shape.split_k;
     const int b1 = bz % shape.nb1, b2 = bz / shape.nb1;
 
-    const int kb_total = (shape.K + GEMM_BK - 1) / GEMM_BK;
+    const int kb_total = (shape.K + S::BK - 1) / S::BK;
     const int kb_per = (kb_total + shape.split_k - 1) / shape.split_k;
     const int kb_begin = split * kb_per;
     const int num_kb = max(0, min(kb_total, kb_begin + kb_per) - kb_begin);
@@ -467,16 +479,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (warp == 8) {
         // ===================== TMA producer: the hi and lo planes of a tile arrive with ONE 3-D box =====================
         if (lane == 0) {
-            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(GEMM_A_TILE + S::B_TILE);
+            const uint32_t stage_bytes = (lo_pass ? 2u : 1u) * (uint32_t)(S::A_TILE + S::B_TILE);
             for (int i = 0; i < num_kb; ++i) {
                 const int s = i % STAGES;
                 mbar_wait(smem_u32(&empty_bar[s]), ((uint32_t)(i / STAGES) & 1u) ^ 1u);
                 const uint32_t fb = smem_u32(&full_bar[s]);
                 const uint32_t sa = smem_base + s * S::STAGE;
-                const int k0 = (kb_begin + i) * GEMM_BK;
+                const int k0 = (kb_begin + i) * S::BK;
                 mbar_arrive_expect_tx(fb, stage_bytes);
                 tma_load_5d(sa, &tmap_a, fb, k0, m_tile * GEMM_BM, 0, b1, b2);
-                tma_load_5d(sa + 2 * GEMM_A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
+                tma_load_5d(sa + 2 * S::A_TILE, &tmap_b, fb, k0, n_tile * BN, 0, b1, b2);
             }
         }
         return;
@@ -489,11 +501,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     for (int i = 0; i < num_kb; ++i) {
         const int s = i % STAGES;
         mbar_wait(smem_u32(&full_bar[s]), (uint32_t)(i / STAGES) & 1u);
-        const uint32_t sa = smem_base + s * S::STAGE + wg * (GEMM_A_TILE / 2);  // this warpgroup's 64 rows
-        const uint32_t sb = smem_base + s * S::STAGE + 2 * GEMM_A_TILE;
+        const uint32_t sa = smem_base + s * S::STAGE + wg * (S::A_TILE / 2);  // this warpgroup's 64 rows
+        const uint32_t sb = smem_base + s * S::STAGE + 2 * S::A_TILE;
         fence_acc(acc);
         wgmma_fence();
-        gemm_kblock<BN>(acc, sa, sa + GEMM_A_TILE, sb, sb + S::B_TILE, lo_pass);
+        gemm_kblock<BN, S::BK>(acc, sa, sa + S::A_TILE, sb, sb + S::B_TILE, lo_pass);
         wgmma_commit();
         wgmma_wait<1>();  // the k-block before this one has retired: release its stage
         fence_acc(acc);
@@ -620,7 +632,7 @@ gemm_rowln_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             for (int kb = 0; kb < 2; ++kb) {
                 if (kb == KB) break;
                 const uint32_t sa = sA + kb * 2 * RL_A_TILE + wg * (RL_A_TILE / 2), sw = sW + kb * 2 * RL_W_TILE;
-                gemm_kblock<256>(acc, sa, sa + RL_A_TILE, sw, sw + RL_W_TILE, lo_pass);
+                gemm_kblock<256, 64>(acc, sa, sa + RL_A_TILE, sw, sw + RL_W_TILE, lo_pass);
             }
             wgmma_commit();
             wgmma_wait<0>();
@@ -717,7 +729,8 @@ static PFN_encodeTiled get_encode() {
     return fn;
 }
 
-static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes = 1) {
+// Boxes of box_k = 64 bf16 along K are 128B-swizzled, boxes of 32 64B-swizzled (one swizzle row per box row).
+static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes, int box_k) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) return PSAM_ERR_UNSUPPORTED;
     const int nb1 = op->nb1 > 0 ? op->nb1 : 1, nb2 = op->nb2 > 0 ? op->nb2 : 1;
@@ -729,22 +742,22 @@ static int make_operand_map(CUtensorMap* map, const psam_operand* op, int box_ro
     for (int i = 0; i < 4; ++i)
         if (strides[i] % 16) return PSAM_ERR_ARG;
     if (((uintptr_t)op->hi) % 16) return PSAM_ERR_ARG;
-    cuuint32_t box[5] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1, 1};
+    cuuint32_t box[5] = {(cuuint32_t)box_k, (cuuint32_t)box_rows, (cuuint32_t)box_planes, 1, 1};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
     CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(op->hi), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, box_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? PSAM_OK : (int)(1000 + r);
 }
 
 int make_operand_map_ext(CUtensorMap* map, const psam_operand* op, int box_rows, int box_planes) {
-    return make_operand_map(map, op, box_rows, box_planes);
+    return make_operand_map(map, op, box_rows, box_planes, 64);
 }
 
-template <int BN, int STAGES>
+template <int BN>
 static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmShape& sh, const GemmEpilogue& ep, cudaStream_t stream) {
-    auto kern = gemm_wgmma_kernel<BN, STAGES>;
-    using S = GemmSmem<BN, STAGES>;
+    auto kern = gemm_wgmma_kernel<BN>;
+    using S = GemmSmem<BN>;
     PSAM_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     const dim3 grid((unsigned)ceil_div(sh.N, BN), (unsigned)ceil_div(sh.M, GEMM_BM), (unsigned)(sh.nb1 * sh.nb2 * sh.split_k));
     PSAM_CUDA_TRY(psam::launch(kern, grid, dim3(GEMM_THREADS), (size_t)S::TOTAL, stream, ma, mb, sh, ep));
@@ -757,7 +770,7 @@ static int launch_gemm(const CUtensorMap& ma, const CUtensorMap& mb, const GemmS
 // the total SM-time instead, which favours wide tiles (fewer operand bytes per flop).
 static int choose_bn(int M, int N, int K, int batches, int split_k, bool throughput) {
     const int mt = ceil_div(M, GEMM_BM);
-    const int kb = ceil_div(ceil_div(K, GEMM_BK), split_k);
+    const int kb = ceil_div(ceil_div(K, 64), split_k);  // 64-wide k-slices
     int best = 128;
     double best_cost = 1e30;
     for (int bn = 64; bn <= 256; bn *= 2) {
@@ -830,13 +843,13 @@ extern "C" int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, co
     if (o->tile_hint >= 32 && o->tile_hint <= 256 && o->tile_hint % 32 == 0) bn = o->tile_hint <= 64 ? 64 : (o->tile_hint <= 128 ? 128 : 256);
     sh.bn = bn;
     CUtensorMap ma, mb;
-    int rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1);
+    int rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1, gemm_bk(bn));
     if (rc) return rc;
-    rc = make_operand_map(&mb, w, bn, passes == 3 ? 2 : 1);
+    rc = make_operand_map(&mb, w, bn, passes == 3 ? 2 : 1, gemm_bk(bn));
     if (rc) return rc;
-    if (bn == 64) return launch_gemm<64, 4>(ma, mb, sh, ep, stream);
-    if (bn == 128) return launch_gemm<128, 3>(ma, mb, sh, ep, stream);
-    return launch_gemm<256, 2>(ma, mb, sh, ep, stream);
+    if (bn == 64) return launch_gemm<64>(ma, mb, sh, ep, stream);
+    if (bn == 128) return launch_gemm<128>(ma, mb, sh, ep, stream);
+    return launch_gemm<256>(ma, mb, sh, ep, stream);
 }
 
 extern "C" int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand* w, const float* gbias, long long ld_gbias, int group_rows,
@@ -856,9 +869,9 @@ extern "C" int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand*
     p.gamma = gamma, p.beta = beta, p.eps = eps, p.act = act;
     p.out_hi = (__nv_bfloat16*)out_hi, p.out_plane = out_plane, p.ldo_s = ldo_s;
     CUtensorMap ma, mw;
-    int rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1);
+    int rc = make_operand_map(&ma, a, GEMM_BM, passes == 3 ? 2 : 1, 64);
     if (rc) return rc;
-    rc = make_operand_map(&mw, w, 256, passes == 3 ? 2 : 1);
+    rc = make_operand_map(&mw, w, 256, passes == 3 ? 2 : 1, 64);
     if (rc) return rc;
     int nsm = 132, devid = 0;
     if (cudaGetDevice(&devid) == cudaSuccess) cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, devid);

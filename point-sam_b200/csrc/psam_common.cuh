@@ -268,6 +268,16 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t
 __device__ __forceinline__ uint64_t gmma_desc_k(uint32_t smem_addr) { return gmma_desc_sw128(smem_addr, 16, 1024); }
 // MN-major tile whose N extent is one 64-element atom: both offsets name the 1024-byte step along K
 __device__ __forceinline__ uint64_t gmma_desc_mn64(uint32_t smem_addr) { return gmma_desc_sw128(smem_addr, 1024, 1024); }
+// 64-byte swizzle, K-major rows of 32 bf16 (64 B): 8-row groups 512 B apart, `lbo` unused.  Tile bases must be 512-byte
+// aligned; advancing the start address by 32 B steps 16 elements along K.
+__device__ __forceinline__ uint64_t gmma_desc_k_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;  // SWIZZLE_64B
+    return d;
+}
 
 // D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both K-major in shared memory; scale_d = 0 overwrites D.
 template <int N>
