@@ -277,6 +277,15 @@ int psam_interp_ln_gelu(const float* f, int Z, int rep, int G, int D, const long
                         const float* gamma, const float* beta, float eps, void* y_hi, long long y_plane,
                         long long ldy_s, cudaStream_t stream);
 
+/* psam_interp_ln_gelu with a per-cloud row addend before the LayerNorm:
+ * y[z*N+n,:] = GELU(LN(sum_k w[b,n,k]*f[z,idx[b,n,k],:] + addend[b,n,:])), b = z/rep, addend fp32 [B,N,D].
+ * Replaces the first stage of MaskDecoderHier's upscaling (mask_decoder.py:322-323): interpolate_features to the level-1
+ * centres, cat with the tokenizer's level-1 embeddings, output_upscaling2[0..2], where output_upscaling2[0] has been split
+ * into its interpolated half (applied to the patch features, f) and its embedding half (applied once per cloud, addend). */
+int psam_interp_add_ln_gelu(const float* f, int Z, int rep, int G, int D, const long long* idx, const float* w, int N,
+                            const float* addend, const float* gamma, const float* beta, float eps, void* y_hi,
+                            long long y_plane, long long ldy_s, cudaStream_t stream);
+
 /* masks[z,c,n] = sum_d hyper[z,c,d] * u[z*N+n,d]  (mask_decoder.py:176). */
 int psam_mask_dot(const float* u, long long ldu, const float* hyper, int Z, int C, int N, int D, float* masks,
                   cudaStream_t stream);

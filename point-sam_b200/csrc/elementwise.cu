@@ -571,12 +571,13 @@ __global__ void decoder_prepare_kernel(const float* __restrict__ iou_token, cons
     }
 }
 
-// one warp per point; D % 128 == 0, D <= 1024: lane owns float4 columns 4*lane + 128*i (128-bit loads, 64-bit split stores)
-template <int NV>
+// one warp per point; D % 128 == 0, D <= 1024: lane owns float4 columns 4*lane + 128*i (128-bit loads, 64-bit split stores).
+// ADD: a per-cloud row addend [B, N, D] (row (z / rep) * N + n) joins the interpolated value before the LayerNorm.
+template <int NV, bool ADD = false>
 __global__ void __launch_bounds__(256)
 interp_ln_gelu_kernel(const float* __restrict__ f, int Z, int rep, int G, int D, const long long* __restrict__ idx,
                       const float* __restrict__ w, int N, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
-                      __nv_bfloat16* __restrict__ yh, long long y_plane, long long ldy_s) {
+                      __nv_bfloat16* __restrict__ yh, long long y_plane, long long ldy_s, const float* __restrict__ addend) {
     pdl_prologue();
     const int wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
     const long long total = (long long)Z * N;
@@ -599,6 +600,10 @@ interp_ln_gelu_kernel(const float* __restrict__ f, int Z, int rep, int G, int D,
             v[i].y = (a.y * w0 + b.y * w1) + d.y * w2;
             v[i].z = (a.z * w0 + b.z * w1) + d.z * w2;
             v[i].w = (a.w * w0 + b.w * w1) + d.w * w2;
+            if constexpr (ADD) {
+                const float4 e = *reinterpret_cast<const float4*>(addend + (o3 / 3) * D + c);
+                v[i].x += e.x; v[i].y += e.y; v[i].z += e.z; v[i].w += e.w;
+            }
             s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
         }
         const float mean = warp_sum(s) / (float)D;
@@ -1111,7 +1116,27 @@ extern "C" int psam_interp_ln_gelu(const float* f, int Z, int rep, int G, int D,
     if (D % 128 || D > 1024 || (ldy_s & 3) || (y_plane & 3)) return PSAM_ERR_UNSUPPORTED;
     const dim3 grid(grid_for((long long)Z * N, 8)), block(256);
     __nv_bfloat16* yh = (__nv_bfloat16*)y_hi;
-#define PSAM_INT(NV) PSAM_CUDA_TRY(psam::launch(interp_ln_gelu_kernel<NV>, grid, block, (size_t)0, stream, f, Z, rep, G, D, idx, w, N, gamma, beta, eps, yh, y_plane, ldy_s))
+#define PSAM_INT(NV) PSAM_CUDA_TRY(psam::launch(interp_ln_gelu_kernel<NV>, grid, block, (size_t)0, stream, f, Z, rep, G, D, idx, w, N, gamma, beta, eps, yh, y_plane, ldy_s, (const float*)nullptr))
+    switch (D / 128) {
+        case 1: PSAM_INT(1); break;
+        case 2: PSAM_INT(2); break;
+        case 4: PSAM_INT(4); break;
+        case 8: PSAM_INT(8); break;
+        default: return PSAM_ERR_UNSUPPORTED;
+    }
+#undef PSAM_INT
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" int psam_interp_add_ln_gelu(const float* f, int Z, int rep, int G, int D, const long long* idx, const float* w, int N,
+                                       const float* addend, const float* gamma, const float* beta, float eps, void* y_hi,
+                                       long long y_plane, long long ldy_s, cudaStream_t stream) {
+    if (!f || !idx || !w || !addend || !gamma || !beta || !y_hi || Z <= 0 || rep <= 0 || D <= 0) return PSAM_ERR_ARG;
+    if (D % 128 || D > 1024 || (ldy_s & 3) || (y_plane & 3)) return PSAM_ERR_UNSUPPORTED;
+    const dim3 grid(grid_for((long long)Z * N, 8)), block(256);
+    __nv_bfloat16* yh = (__nv_bfloat16*)y_hi;
+#define PSAM_INT(NV) PSAM_CUDA_TRY(psam::launch(interp_ln_gelu_kernel<NV, true>, grid, block, (size_t)0, stream, f, Z, rep, G, D, idx, w, N, gamma, beta, eps, yh, y_plane, ldy_s, addend))
     switch (D / 128) {
         case 1: PSAM_INT(1); break;
         case 2: PSAM_INT(2); break;

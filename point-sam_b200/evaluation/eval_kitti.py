@@ -67,8 +67,11 @@ def parse_rotation(spec: Optional[str]) -> Optional[np.ndarray]:
 
 
 def set_group_shape(model, num_points: int):
-    """eval_kitti.py:352-362: the tokenizer's group count / size are runtime attributes chosen per cloud."""
-    g = model.pc_encoder.patch_embed.grouper
+    """eval_kitti.py:352-362: the tokenizer's group count / size are runtime attributes chosen per cloud.  A hierarchical
+    tokenizer (PatchEmbedHier: grouper1 / grouper2, which that override does not address) is left as configured."""
+    g = getattr(model.pc_encoder.patch_embed, "grouper", None)
+    if g is None:
+        return
     if num_points > 30000:
         g.num_groups, g.group_size = 2048, 256
     else:

@@ -38,22 +38,37 @@ class PointCloudSAM(nn.Module):
         pc_pe = engine.run_pos_embedding(self.point_encoder.pe_layer, centers, check=False)
         return dict(pc_embeddings=pc_embeddings, patches=patches, aux=aux, pc_pe=pc_pe, coords=coords)
 
-    def _decode(self, enc, prompt_coords, prompt_labels, prompt_masks, multimask_output, center_idx=None):
+    def _decode_unchecked(self, enc, prompt_coords, prompt_labels, prompt_masks, multimask_output, center_idx=None):
         patches = enc["patches"]
         sparse = engine.run_point_encoder(self.point_encoder, prompt_coords, prompt_labels, check=False)
         dense = self.mask_encoder(prompt_masks, enc["coords"], patches["centers"], patches["knn_idx"], center_idx=center_idx)
         if prompt_masks is not None:
             dense = repeat_interleave(dense, sparse.shape[0] // dense.shape[0], 0)
-        masks, iou = self.mask_decoder(enc["pc_embeddings"], enc["pc_pe"], sparse, dense, aux_inputs=enc["aux"],
-                                       multimask_output=multimask_output)
+        return self.mask_decoder(enc["pc_embeddings"], enc["pc_pe"], sparse, dense, aux_inputs=enc["aux"],
+                                 multimask_output=multimask_output)
+
+    def _decode(self, enc, prompt_coords, prompt_labels, prompt_masks, multimask_output, center_idx=None):
+        masks, iou = self._decode_unchecked(enc, prompt_coords, prompt_labels, prompt_masks, multimask_output, center_idx)
         engine.raise_if_out_of_range(masks.device)  # ValueError like prompt_encoder.py:44-46 (one host sync)
         return masks, iou
+
+    def _center_idx(self, enc):
+        """FPS indices of the centres, for MaskEncoder(centralize_features=True)."""
+        return enc["patches"].get("fps_idx")
+
+    def _group_shape(self) -> tuple:
+        g = self.pc_encoder.patch_embed.grouper
+        return g.num_groups, g.group_size
+
+    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval):
+        from .prompt_sampling import sample_prompts_adapter
+
+        return sample_prompts_adapter(coords, gt_masks, prompt_masks, is_eval=is_eval)
 
     # ------------------------------------------------------------------------------------------
     def set_pointcloud(self, xyz: torch.Tensor, rgb: torch.Tensor):
         """demo/app.py:199 - encode once, keep the embeddings for subsequent prompt decodes."""
-        key = (xyz.data_ptr(), xyz._version, tuple(xyz.shape), rgb.data_ptr(), rgb._version,
-               self.pc_encoder.patch_embed.grouper.num_groups, self.pc_encoder.patch_embed.grouper.group_size)
+        key = (xyz.data_ptr(), xyz._version, tuple(xyz.shape), rgb.data_ptr(), rgb._version) + self._group_shape()
         if self._cloud is not None and self._cloud_key == key:
             return  # same tensors, unmodified: keep the embeddings (the demo calls this on every click)
         with torch.no_grad():
@@ -120,7 +135,7 @@ class PointCloudSAM(nn.Module):
         for t in range(len(prompt_coords_seq)):
             pc = torch.cat([pc, prompt_coords_seq[t]], dim=1)
             pl = torch.cat([pl, prompt_labels_seq[t]], dim=1)
-            masks, iou = self._decode(enc, pc, pl, pm, t == 0, center_idx=enc["patches"].get("fps_idx"))
+            masks, iou = self._decode(enc, pc, pl, pm, t == 0, center_idx=self._center_idx(enc))
             if t == 0:
                 best = torch.argmax(iou, dim=1)
                 pm = batch_index_select(masks, best, dim=1)
@@ -135,8 +150,6 @@ class PointCloudSAM(nn.Module):
         """Reference forward (pc_sam.py:90-196); also accepts the xyz/rgb/mask spelling used by
         evaluation/inference.py:67-68.  Prompts are sampled from the ground truth with the reference's
         sampler (pc_sam/model/common.py:287-474) restated in pc_sam.model.prompt_sampling."""
-        from .prompt_sampling import sample_prompts_adapter
-
         if self.training:
             # the reference's train() branch (pc_sam.py:150-165: mask-refinement iterations without new prompts, random
             # prompt sampler, autograd) is not part of this inference-only path; fail instead of silently doing eval
@@ -155,10 +168,10 @@ class PointCloudSAM(nn.Module):
         pl = gt_masks.new_empty((B * M, 0))
         pm = None
         for i in range(self.prompt_iters):
-            npc, npl = sample_prompts_adapter(coords, gt_masks, pm, is_eval=is_eval)
+            npc, npl = self._sample_prompts(coords, gt_masks, pm, is_eval)
             pc = torch.cat([pc, npc], dim=1)
             pl = torch.cat([pl, npl], dim=1)
-            masks, iou = self._decode(enc, pc, pl, pm, i == 0, center_idx=enc["patches"].get("fps_idx"))
+            masks, iou = self._decode(enc, pc, pl, pm, i == 0, center_idx=self._center_idx(enc))
             if i == 0:
                 best = torch.argmax(iou, dim=1)
                 pm = batch_index_select(masks, best, dim=1)
@@ -173,6 +186,50 @@ class PointCloudSAM(nn.Module):
 PointSAM = PointCloudSAM
 
 
+class PointCloudSAMHier(PointCloudSAM):
+    """PointCloudSAMHier (/root/reference/pc_sam/model/pc_sam.py:377-496): PatchEmbedHier tokenizer, MaskEncoderHier and
+    MaskDecoderHier; the transformer sees the level-2 patches, the decoder upscales level 2 -> level 1 -> points.
+
+    forward(is_eval=False) is the reference's loop (random prompt of the error region every round, pc_sam.py:434).
+    Extensions over the reference, where its inherited methods fail: forward(is_eval=True) uses the ground-truth border
+    sampler exactly as PointCloudSAM.forward(is_eval=True) (so the evaluation driver and the iterative graph predictor run
+    this model), and predict_masks / predict_iterative / set_pointcloud run one round of the forward loop body with the
+    given prompts (the reference's inherited predict_masks indexes the list of patch levels with a string, pc_sam.py:54)."""
+
+    def _encode(self, coords, features):
+        pc_embeddings, patches = self.pc_encoder(coords, features)
+        p1, p2 = patches
+        aux1 = AuxInputs(coords=coords, features=features, centers=p1["centers"])
+        aux2 = AuxInputs(coords=p1["centers"], features=p1["embeddings"], centers=p2["centers"])
+        engine.hier_embedding_term(self.mask_decoder, aux2)  # per cloud: kept by set_pointcloud across prompts
+        pc_pe = engine.run_pos_embedding(self.point_encoder.pe_layer, p2["centers"], check=False)
+        return dict(pc_embeddings=pc_embeddings, patches=patches, aux=(aux1, aux2), pc_pe=pc_pe, coords=coords)
+
+    def _decode_unchecked(self, enc, prompt_coords, prompt_labels, prompt_masks, multimask_output, center_idx=None):
+        p1, p2 = enc["patches"]
+        sparse = engine.run_point_encoder(self.point_encoder, prompt_coords, prompt_labels, check=False)
+        dense = self.mask_encoder(prompt_masks, enc["coords"], p1["centers"], p1["knn_idx"], p2["centers"], p2["knn_idx"])
+        if isinstance(dense, list):  # pc_sam.py:452-460: the last level, already batched B*M
+            dense = dense[-1]
+        aux1, aux2 = enc["aux"]
+        return self.mask_decoder(enc["pc_embeddings"], enc["pc_pe"], sparse, dense, aux_inputs1=aux1, aux_inputs2=aux2,
+                                 multimask_output=multimask_output)
+
+    def _center_idx(self, enc):
+        return None  # MaskEncoderHier has no centralize_features
+
+    def _group_shape(self) -> tuple:
+        pe = self.pc_encoder.patch_embed
+        return pe.grouper1.num_groups, pe.grouper1.group_size, pe.grouper2.num_groups, pe.grouper2.group_size
+
+    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval):
+        if is_eval:
+            return super()._sample_prompts(coords, gt_masks, prompt_masks, is_eval)
+        from .prompt_sampling import sample_prompts
+
+        return sample_prompts(coords, gt_masks, prompt_masks)
+
+
 def build_point_sam(encoder: str = "eva02_large_patch14_448", num_patches: int = 512, patch_size: int = 64,
                     embed_dim: int = 256, prompt_iters: int = 5) -> PointCloudSAM:
     """Dependency-free mirror of configs/model/{base,default,giant}.yaml (hydra/timm are absent offline)."""
@@ -185,3 +242,20 @@ def build_point_sam(encoder: str = "eva02_large_patch14_448", num_patches: int =
     me = MaskEncoder(embed_dim)
     md = MaskDecoder(embed_dim, TwoWayTransformer(2, embed_dim, 8, 2048))
     return PointCloudSAM(enc, me, md, prompt_iters).eval()
+
+
+def build_point_sam_hier(encoder: str = "eva02_large_patch14_448", num_patches=(2048, 512), patch_size=(32, 32),
+                         radius=(0.05, 0.1), prompt_iters: int = 8, embed_dim: int = 256) -> PointCloudSAMHier:
+    """Dependency-free mirror of configs/model/hier.yaml."""
+    from .eva import create_model
+    from .mask_decoder import MaskDecoderHier
+    from .pc_encoder import PatchEmbedHier
+    from .prompt_encoder import MaskEncoderHier
+    from .transformer import TwoWayTransformer
+
+    radius = list(radius) if radius is not None else None
+    pe = PatchEmbedHier(6, 512, list(num_patches), list(patch_size), radius)
+    enc = PointCloudEncoder(pe, create_model(encoder), embed_dim)
+    me = MaskEncoderHier(embed_dim, radius=radius)
+    md = MaskDecoderHier(embed_dim, TwoWayTransformer(2, embed_dim, 8, 2048))
+    return PointCloudSAMHier(enc, me, md, prompt_iters).eval()

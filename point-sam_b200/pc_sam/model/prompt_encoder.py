@@ -1,7 +1,7 @@
 """/root/reference/pc_sam/model/prompt_encoder.py:13-133."""
 from __future__ import annotations
 
-from typing import Optional, Union
+from typing import List, Optional, Union
 
 import torch
 from torch import nn
@@ -47,3 +47,20 @@ class MaskEncoder(nn.Module):
 
     def forward(self, masks: Union[torch.Tensor, None], coords, centers, knn_idx, center_idx=None) -> torch.Tensor:
         return engine.run_mask_encoder(self, masks, coords, centers, knn_idx, center_idx)
+
+
+class MaskEncoderHier(nn.Module):
+    """/root/reference/pc_sam/model/prompt_encoder.py:136-183 (two-level PointNet++-style mask encoder)."""
+
+    def __init__(self, embed_dim, in_channels=4, radius: Optional[List[float]] = None):
+        super().__init__()
+        self.embed_dim = embed_dim
+        self.in_channels = in_channels
+        self.radius = radius
+        self.patch_encoder1 = PatchEncoder(in_channels, 128, [64, 128])
+        self.patch_encoder2 = PatchEncoder(128 + 3, embed_dim, [128, 256])
+        self.no_mask_embed = nn.Embedding(1, embed_dim)
+
+    def forward(self, masks: Union[torch.Tensor, None], coords, centers1, knn_idx1, centers2, knn_idx2):
+        """No mask: no_mask_embed broadcast over [B, G2, D]; otherwise the list [x1 [B*M, G1, 128], x2 [B*M, G2, D]]."""
+        return engine.run_mask_encoder_hier(self, masks, coords, centers1, knn_idx1, centers2, knn_idx2)

@@ -105,9 +105,11 @@ def compose(config_dir: str, config_name: str, overrides=()) -> Dict:
     return cfg
 
 
-# The three shipped model configurations (configs/model/{base,default,giant}.yaml) as a function of the encoder name,
+# The shipped model configurations (configs/model/{base,default,giant,hier}.yaml) as a function of the encoder name,
 # for hosts without the reference's configs directory.
 def model_config(name: str = "large") -> Dict:
+    if name == "hier":
+        return _hier_config()
     enc = {"base": "eva02_base_patch14_448", "large": "eva02_large_patch14_448", "default": "eva02_large_patch14_448",
            "giant": "eva_giant_patch14_560"}[name]
     G, K, iters = (1024, 256, 5) if name in ("large", "default") else (512, 64, 10)  # as shipped in configs/model/*.yaml
@@ -122,3 +124,21 @@ def model_config(name: str = "large") -> Dict:
                              "transformer": {"_target_": "pc_sam.model.transformer.TwoWayTransformer", "depth": 2,
                                              "embedding_dim": 256, "num_heads": 8, "mlp_dim": 2048}},
             "prompt_iters": iters}
+
+
+def _hier_config() -> Dict:
+    """configs/model/hier.yaml: PointCloudSAMHier with the two-level tokenizer, mask encoder and upscaling decoder."""
+    radius = [0.05, 0.1]
+    return {"_target_": "pc_sam.model.pc_sam.PointCloudSAMHier",
+            "pc_encoder": {"_target_": "pc_sam.model.pc_encoder.PointCloudEncoder",
+                           "patch_embed": {"_target_": "pc_sam.model.pc_encoder.PatchEmbedHier", "in_channels": 6,
+                                           "out_channels": 512, "num_patches": [2048, 512], "patch_size": [32, 32],
+                                           "radius": list(radius)},
+                           "transformer": {"_target_": "timm.create_model", "model_name": "eva02_large_patch14_448",
+                                           "pretrained": False},
+                           "embed_dim": 256},
+            "mask_encoder": {"_target_": "pc_sam.model.prompt_encoder.MaskEncoderHier", "embed_dim": 256, "radius": list(radius)},
+            "mask_decoder": {"_target_": "pc_sam.model.mask_decoder.MaskDecoderHier", "transformer_dim": 256,
+                             "transformer": {"_target_": "pc_sam.model.transformer.TwoWayTransformer", "depth": 2,
+                                             "embedding_dim": 256, "num_heads": 8, "mlp_dim": 2048}},
+            "prompt_iters": 8}

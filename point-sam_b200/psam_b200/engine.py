@@ -243,15 +243,17 @@ def _run_res_blocks(blocks, x: torch.Tensor):
         ops.gemm(un, pb.w2, bias=pb.bb2, out_f32=x, resid=x, passes=PASSES)
 
 
-def run_patch_embed_hier(m, coords, features):
+def run_patch_embed_hier(m, coords, features, want_split: bool = False):
     """PatchEmbedHier.forward (pc_encoder.py:200-239): PointNet++-style two-level tokenizer; the second level groups the
-    first level's centres (already in FPS order: use_fps=False) with the first level's embeddings as features."""
+    first level's centres (already in FPS order: use_fps=False) with the first level's embeddings as features.
+    want_split: also return the split-bf16 copy of the level-2 embeddings (the operand of patch_proj)."""
     patches1 = run_knn_grouper(m.grouper1, coords, features)
     x1 = run_patch_encoder(m.patch_encoder1, patches1["features"])
     patches1["embeddings"] = x1
     patches2 = run_knn_grouper(m.grouper2, patches1["centers"], x1, use_fps=False)
-    patches2["embeddings"] = run_patch_encoder(m.patch_encoder2, patches2["features"])
-    return [patches1, patches2]
+    out = run_patch_encoder(m.patch_encoder2, patches2["features"], want_split=want_split)
+    patches2["embeddings"] = out[0] if want_split else out
+    return ([patches1, patches2], out[1]) if want_split else [patches1, patches2]
 
 
 def run_patch_embed_nn(m, coords, features):
@@ -595,17 +597,25 @@ def _run_mlp_folded(pb: _PackedBlock, x, xs, st_mid, st_out, M, D, dev, stats=No
 
 
 def run_pc_encoder(enc, coords, features):
+    """PointCloudEncoder.forward (pc_encoder.py:118-145).  A hierarchical tokenizer (PatchEmbedHier) returns a list of
+    patch dicts: the transformer consumes the last level's embeddings and centres, and the list is returned."""
     pk = _cached(enc, _PackedEncoder)
-    patches = run_knn_grouper(enc.patch_embed.grouper, coords, features)
-    emb, embs = run_patch_encoder(enc.patch_embed.patch_encoder, patches["features"], want_split=True)
-    patches["embeddings"] = emb
+    if hasattr(enc.patch_embed, "grouper1"):
+        patches, embs = run_patch_embed_hier(enc.patch_embed, coords, features, want_split=True)
+        last = patches[-1]
+    else:
+        patches = run_knn_grouper(enc.patch_embed.grouper, coords, features)
+        emb, embs = run_patch_encoder(enc.patch_embed.patch_encoder, patches["features"], want_split=True)
+        patches["embeddings"] = emb
+        last = patches
+    emb = last["embeddings"]
     B, L, _ = emb.shape
     D, dev = pk.D, emb.device
     M = B * L
     x = torch.empty((M, D), dtype=torch.float32, device=dev)
     ops.gemm(embs, pk.wpp, bias=pk.bpp, out_f32=x, passes=PASSES)
     pos = Split(M, pk.wpos0.shape[0], dev)
-    ops.small_in_linear(patches["centers"], pk.wpos0, pk.bpos0, None, None, 0.0, False, ACT_GELU, pos)
+    ops.small_in_linear(last["centers"], pk.wpos0, pk.bpos0, None, None, 0.0, False, ACT_GELU, pos)
     if pk.fold_block and _use_block_ln_fold():
         # LayerNorm-free encoder: every GEMM that writes the residual stream also writes its split-bf16 copy and row
         # statistics; norm1 / norm2 / fc_norm are applied inside the consuming GEMMs' epilogues
@@ -730,6 +740,20 @@ def run_mask_encoder(me, masks, coords, centers, knn_idx, center_idx=None):
     return run_patch_encoder(me.patch_encoder, groups)
 
 
+def run_mask_encoder_hier(me, masks, coords, centers1, knn_idx1, centers2, knn_idx2):
+    """MaskEncoderHier.forward (prompt_encoder.py:150-183): the prompt-mask logits grouped around the level-1 centres
+    (PatchEncoder(4, 128)), then the level-1 features grouped around the level-2 centres (PatchEncoder(131, D)).  The
+    features are batched B*M, the coordinates B.  Returns [x1 [B*M, G1, 128], x2 [B*M, G2, D]]."""
+    if masks is None:
+        return me.no_mask_embed.weight.reshape(1, 1, -1).expand(centers2.shape[0], centers2.shape[1], -1)
+    r = me.radius
+    m = masks.detach().float().contiguous().unsqueeze(-1)
+    g1 = ops.group_gather(coords.float().contiguous(), m, centers1, knn_idx1, r[0] if r else None)
+    x1 = run_patch_encoder(me.patch_encoder1, g1)
+    g2 = ops.group_gather(centers1, x1, centers2, knn_idx2, r[1] if r else None)
+    return [x1, run_patch_encoder(me.patch_encoder2, g2)]
+
+
 # ------------------------------------------------------------------------------------------------
 # two-way transformer + mask decoder, pc_sam/model/transformer.py, mask_decoder.py
 # ------------------------------------------------------------------------------------------------
@@ -783,14 +807,33 @@ class _PackedDecoder:
         for li in range(3):
             self.hyper.append((torch.stack([_f32(m.layers[li].weight) for m in md.output_hypernetworks_mlps]).contiguous(),
                                torch.stack([_f32(m.layers[li].bias) for m in md.output_hypernetworks_mlps]).contiguous()))
-        up = md.output_upscaling
-        self.up0w, self.up0b = _f32(up[0].weight), _f32(up[0].bias)
-        if DECODER_TC:
-            self.up0w_s = ops.pack_weight(up[0].weight)
-        self.up1 = _ln(up[1])
-        self.up3w, self.up3b = ops.pack_weight(up[3].weight), _f32(up[3].bias)
         self.iou = [(_f32(l.weight), _f32(l.bias)) for l in md.iou_prediction_head.layers]
         self.iou_sigmoid = md.iou_prediction_head.sigmoid_output
+        self.hier = hasattr(md, "output_upscaling2")
+        if not self.hier:
+            up = md.output_upscaling
+            self.up0w, self.up0b = _f32(up[0].weight), _f32(up[0].bias)
+            if DECODER_TC:
+                self.up0w_s = ops.pack_weight(up[0].weight)
+            self.up1 = _ln(up[1])
+            self.up3w, self.up3b = ops.pack_weight(up[3].weight), _f32(up[3].bias)
+            return
+        # MaskDecoderHier (mask_decoder.py:242-254, 322-325).  up2[0] acts on cat([interp(keys), emb1]): its first D columns
+        # commute with the interpolation (the weights sum to 1) and run on the G2 key rows ("up0", as in the base decoder);
+        # the embedding half (+ bias) is per cloud (emb_w / emb_b).  up1[0] o interp o up2[3] = interp o (up1[0] o up2[3]):
+        # one D -> D/2 GEMM at the level-1 rows, the product formed in fp64.
+        up2, up1 = md.output_upscaling2, md.output_upscaling1
+        w20 = up2[0].weight.detach().float()
+        self.up0w, self.up0b = _f32(w20[:, :self.D]), torch.zeros(self.D, dtype=torch.float32, device=w20.device)
+        if DECODER_TC:
+            self.up0w_s = ops.pack_weight(w20[:, :self.D])
+        self.emb_w, self.emb_b = ops.pack_weight(w20[:, self.D:]), _f32(up2[0].bias)
+        self.up2_ln = _ln(up2[1])
+        w10, w23 = up1[0].weight.detach().double(), up2[3].weight.detach().double()
+        self.mid_w = ops.pack_weight((w10 @ w23).float())
+        self.mid_b = (w10 @ up2[3].bias.detach().double() + up1[0].bias.detach().double()).float().contiguous()
+        self.up1 = _ln(up1[1])
+        self.up3w, self.up3b = ops.pack_weight(up1[3].weight), _f32(up1[3].bias)
 
 
 def _attend(pa: _PackedAttn, q_in, q_pe, k_in, k_pe, v_in, Z, Lq, Lk):
@@ -901,8 +944,9 @@ def _run_decoder_tc(pk, queries, keys, qpe, pe_z, aux, Z, T, G, D, rep, ids, mas
 
 def _decoder_heads(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev):
     """mask_decoder.py:146-184: upsampling, hyper-network product, IoU head.  f0 = output_upscaling[0](keys) [Z*G, D]."""
+    if pk.hier:
+        return _decoder_heads_hier(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev)
     hs = queries  # [Z*T, D]
-    C = len(ids)
     # upscaling (mask_decoder.py:146-164): Linear0 commutes with the (affine, weights sum to 1) interpolation
     if aux.interp_index is None or aux.interp_weight is None:
         aux.interp_index, aux.interp_weight = ops.knn3_interp(aux.coords.float().contiguous(), aux.centers)
@@ -911,6 +955,13 @@ def _decoder_heads(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev):
     nv.check(nv.lib().psam_interp_ln_gelu(nv.ptr(f0), Z, rep, G, D, nv.ptr(aux.interp_index), nv.ptr(aux.interp_weight), N,
                                           nv.ptr(pk.up1[0]), nv.ptr(pk.up1[1]), pk.up1[2], u1.ptr(), u1.plane, u1.pitch,
                                           nv.stream()), "interp_ln_gelu")
+    return _mask_heads(pk, hs, u1, Z, T, N, D, ids, mask_slice, dev)
+
+
+def _mask_heads(pk, hs, u1, Z, T, N, D, ids, mask_slice, dev):
+    """Hyper-network MLPs, last upscaling Linear + GELU dotted with them (mask_decoder.py:163-176), IoU head (:180-182).
+    u1: split-bf16 [Z*N, Du] input of the last upscaling Linear (Du = D, or D/2 for MaskDecoderHier)."""
+    C = len(ids)
     # hyper-network MLPs on the selected mask tokens (mask_decoder.py:167-175), batched over tokens
     i0 = ids[0]
     x = hs
@@ -918,19 +969,21 @@ def _decoder_heads(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev):
     xoff = (1 + i0) * D
     hyper = None
     for li, (w, b) in enumerate(pk.hyper):
-        y = torch.empty((Z, C, D), dtype=torch.float32, device=dev)
-        ops.linear_f32(x, w[i0:i0 + C], b[i0:i0 + C], act=ACT_RELU if li < 2 else ACT_NONE, out=y, M=Z, K=D, ldx=ld, Z=C,
-                       x_z=D, w_z=D * D, b_z=D, y_z=D, ldy=C * D, x_off=xoff)
-        x, ld, xoff, hyper = y, C * D, 0, y
+        Do, Ki = w.shape[1], w.shape[2]
+        y = torch.empty((Z, C, Do), dtype=torch.float32, device=dev)
+        ops.linear_f32(x, w[i0:i0 + C], b[i0:i0 + C], act=ACT_RELU if li < 2 else ACT_NONE, out=y, M=Z, K=Ki, ldx=ld, Z=C,
+                       x_z=Ki, w_z=Do * Ki, b_z=Do, y_z=Do, ldy=C * Do, x_off=xoff)
+        x, ld, xoff, hyper = y, C * Do, 0, y
+    Du = pk.up3w.rows
     if FUSED_MASK_DOT and N % 32 == 0 and C <= 8:
         # output_upscaling[3..4] (Linear + GELU) and the hyper-network product fused into one GEMM epilogue
         masks = torch.zeros((Z, C, N), dtype=torch.float32, device=dev)
         ops.gemm(u1, pk.up3w, bias=pk.up3b, act=ACT_GELU, passes=PASSES, rowdot=(hyper, masks))
     else:
-        u2 = torch.empty((Z * N, D), dtype=torch.float32, device=dev)
+        u2 = torch.empty((Z * N, Du), dtype=torch.float32, device=dev)
         ops.gemm(u1, pk.up3w, bias=pk.up3b, out_f32=u2, act=ACT_GELU, passes=PASSES)
         masks = torch.empty((Z, C, N), dtype=torch.float32, device=dev)
-        nv.check(nv.lib().psam_mask_dot(nv.ptr(u2), D, nv.ptr(hyper), Z, C, N, D, nv.ptr(masks), nv.stream()), "mask_dot")
+        nv.check(nv.lib().psam_mask_dot(nv.ptr(u2), Du, nv.ptr(hyper), Z, C, N, Du, nv.ptr(masks), nv.stream()), "mask_dot")
 
     # IoU head on the iou token (mask_decoder.py:180-182)
     y = hs
@@ -941,3 +994,49 @@ def _decoder_heads(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev):
     if pk.iou_sigmoid:
         y = torch.sigmoid(y)
     return masks, y[:, mask_slice].contiguous()
+
+
+def hier_embedding_term(md, aux2):
+    """MaskDecoderHier: output_upscaling2[0]'s embedding half + bias on the tokenizer's level-1 embeddings, [B*G1, D]: once
+    per encoded cloud (cached on aux_inputs2 like its interpolation weights)."""
+    return _hier_embedding_term(_cached(md, _PackedDecoder), aux2)
+
+
+def _hier_embedding_term(pk, aux2):
+    e = getattr(aux2, "_psam_emb_term", None)
+    if e is None:
+        feats = aux2.features.float().contiguous()
+        B, G1, Ce = feats.shape
+        fs = Split(B * G1, Ce, feats.device)
+        ops.split_f32(feats.view(B * G1, Ce), fs)
+        e = torch.empty((B * G1, pk.D), dtype=torch.float32, device=feats.device)
+        ops.gemm(fs, pk.emb_w, bias=pk.emb_b, out_f32=e, passes=PASSES)
+        aux2._psam_emb_term = e
+    return e
+
+
+def _decoder_heads_hier(pk, queries, f2, aux, Z, T, G2, D, rep, ids, mask_slice, dev):
+    """MaskDecoderHier upscaling (mask_decoder.py:322-325): patches -> level-1 centres -> points.
+    f2 = keys @ output_upscaling2[0].weight[:, :D]^T [Z*G2, D]; aux = (aux_inputs1: points <- level-1 centres,
+    aux_inputs2: level-1 <- level-2 centres)."""
+    aux1, aux2 = aux
+    for a in (aux1, aux2):
+        if a.interp_index is None or a.interp_weight is None:
+            a.interp_index, a.interp_weight = ops.knn3_interp(a.coords.float().contiguous(), a.centers.float().contiguous())
+    e = _hier_embedding_term(pk, aux2)
+    G1, N = aux2.coords.shape[1], aux1.coords.shape[1]
+    # interp(f2) + e -> LayerNorm -> GELU at the level-1 rows
+    h = Split(Z * G1, D, dev)
+    g, b, eps = pk.up2_ln
+    nv.check(nv.lib().psam_interp_add_ln_gelu(nv.ptr(f2), Z, rep, G2, D, nv.ptr(aux2.interp_index), nv.ptr(aux2.interp_weight),
+                                              G1, nv.ptr(e), nv.ptr(g), nv.ptr(b), eps, h.ptr(), h.plane, h.pitch,
+                                              nv.stream()), "interp_add_ln_gelu")
+    # output_upscaling1[0] o output_upscaling2[3] at the level-1 rows, then interp to the points -> LayerNorm -> GELU
+    Dh = pk.mid_w.rows
+    f1 = torch.empty((Z * G1, Dh), dtype=torch.float32, device=dev)
+    ops.gemm(h, pk.mid_w, bias=pk.mid_b, out_f32=f1, passes=PASSES)
+    u1 = Split(Z * N, Dh, dev)
+    nv.check(nv.lib().psam_interp_ln_gelu(nv.ptr(f1), Z, rep, G1, Dh, nv.ptr(aux1.interp_index), nv.ptr(aux1.interp_weight), N,
+                                          nv.ptr(pk.up1[0]), nv.ptr(pk.up1[1]), pk.up1[2], u1.ptr(), u1.plane, u1.pitch,
+                                          nv.stream()), "interp_ln_gelu")
+    return _mask_heads(pk, queries, u1, Z, T, N, D, ids, mask_slice, dev)

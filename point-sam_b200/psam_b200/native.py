@@ -61,7 +61,7 @@ EXPORTS = [
     "psam_border_prompt_workspace_bytes", "psam_border_prompt_f32",
     "psam_gemm_bf16x3", "psam_gemm_rowln_bf16x3", "psam_attention_bf16x3", "psam_attention_bf16x3_twopass", "psam_linear_f32", "psam_layernorm_f32", "psam_swiglu_ln", "psam_small_in_linear",
     "psam_group_max", "psam_softmax_split", "psam_transpose_split", "psam_posenc_f32", "psam_attention_f32",
-    "psam_decoder_prepare", "psam_interp_ln_gelu", "psam_mask_dot", "psam_add_bcast_f32", "psam_split_f32", "psam_split_add_f32",
+    "psam_decoder_prepare", "psam_interp_ln_gelu", "psam_interp_add_ln_gelu", "psam_mask_dot", "psam_add_bcast_f32", "psam_split_f32", "psam_split_add_f32",
     "psam_version",
 ]
 
@@ -104,6 +104,7 @@ def lib():
             "psam_attention_f32": [p, p, p, p, i, i, i, i, i, ll, ll, ll, ll, p],
             "psam_decoder_prepare": [p, p, i, p, i, p, p, ll, ll, i, i, i, i, p, p, p],
             "psam_interp_ln_gelu": [p, i, i, i, i, p, p, i, p, p, f, p, ll, ll, p],
+            "psam_interp_add_ln_gelu": [p, i, i, i, i, p, p, i, p, p, p, f, p, ll, ll, p],
             "psam_mask_dot": [p, ll, p, i, i, i, i, p, p],
             "psam_add_bcast_f32": [p, p, ll, ll, ll, ll, p, p],
             "psam_split_f32": [p, ll, ll, i, p, ll, ll, ll, p],

@@ -47,10 +47,7 @@ class GraphPredictor:
             enc = self.model._encode(self.xyz, self.feats)
             return enc["pc_embeddings"], enc["pc_pe"]
         enc = self.model._encode(self.xyz, self.feats)
-        sparse = engine.run_point_encoder(self.model.point_encoder, self.pc, self.pl, check=False)
-        dense = self.model.mask_encoder(None, self.xyz, enc["patches"]["centers"], enc["patches"]["knn_idx"])
-        return self.model.mask_decoder(enc["pc_embeddings"], enc["pc_pe"], sparse, dense, aux_inputs=enc["aux"],
-                                       multimask_output=self.multimask)
+        return self.model._decode_unchecked(enc, self.pc, self.pl, None, self.multimask)
 
     def warmup(self, xyz, feats, pc, pl):
         """Eager passes (pack weights, size the allocator) then capture."""
