@@ -299,6 +299,42 @@ int psam_add_bcast_f32(const float* a, const float* b, long long n, long long ch
 int psam_split_f32(const float* x, long long ld, long long rows, int D, void* y_hi, long long y_plane,
                    long long ldy_s, long long pitch, cudaStream_t stream);
 
+/* ---- automatic mask generation ("segment everything") ------------------------------------------ */
+
+/* Candidate extraction of a batch of multimask decoder outputs.  Stands in for the filtering stage of segment-anything's
+ * SamAutomaticMaskGenerator._process_batch (predicted-IoU filter, stability score, binarisation), restated for point
+ * clouds; the caller loops over prompt batches and gives every batch its own `base`.
+ * logits [Z, C, N] fp32, iou_preds [Z, C] fp32.  Each logit row is read once (128-bit loads when N % 4 == 0 and the
+ * pointer is 16-byte aligned).  Candidate slot s = base + z*C + c receives
+ *   bits[s*W .. s*W+W)  the bit-packed mask logit > mask_threshold (point n = bit n%32 of word n/32; words past N zero),
+ *   area[s]             the number of set bits (int32),
+ *   stability[s]        fp32(count(logit > hi)) / fp32(count(logit > lo)) with IEEE division (0/0 = NaN), where
+ *                       hi = mask_threshold + stability_offset and lo = mask_threshold - stability_offset in fp32,
+ *   score[s]            iou_preds[z, c] if the candidate survives, -inf if it does not.
+ * A candidate survives when all of these hold (SAM's comparisons):
+ *   iou > pred_iou_thresh          (only when pred_iou_thresh > 0; a NaN IoU never survives),
+ *   stability >= stability_thresh  (only when stability_thresh > 0),
+ *   area >= min_area, and area >= 1 (an empty mask is never kept).
+ * W >= ceil(N/32).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z, int C, int N, float mask_threshold,
+                             float stability_offset, float pred_iou_thresh, float stability_thresh, int min_area,
+                             long long base, int W, uint32_t* bits, int* area, float* stability, float* score,
+                             cudaStream_t stream);
+
+/* Greedy mask-IoU non-maximum suppression over K <= 16384 candidate slots of W words each (the output of
+ * psam_mask_candidates_f32).  Stands in for the duplicate-removal stage of SamAutomaticMaskGenerator._process_batch /
+ * _process_crop (batched_nms on boxes), here on the masks themselves.
+ * Candidates are ordered by (score descending, slot index ascending); -inf scores are dropped.  Walking that order, a
+ * candidate is kept unless an earlier kept one overlaps it with
+ *   fp32(inter) / fp32(area_i + area_j - inter) > nms_thresh,   inter = popcount(bits_i & bits_j),
+ * so the result is exact and bit-reproducible.  Three launches (order, pairwise suppression bits, greedy scan) and no
+ * host synchronisation: the number of valid candidates stays on the device.
+ * Outputs: keep[0 .. *keep_count) = the kept slot indices in score order (keep holds K ints), *keep_count (device int32).
+ * bits / area / score may be NULL when K == 0.  workspace: psam_mask_nms_workspace_bytes(K, W) bytes, 16-byte aligned. */
+size_t psam_mask_nms_workspace_bytes(int K, int W);
+int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh, int* keep,
+                  int* keep_count, void* workspace, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

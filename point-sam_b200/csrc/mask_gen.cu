@@ -1,0 +1,365 @@
+// Automatic mask generation ("segment everything"): candidate extraction from multimask decoder logits and greedy
+// mask-IoU NMS, all on the device.  The semantics are stated in include/psam_b200.h.
+//
+//   mask_candidates_kernel   one CTA per logit row: a single streaming pass (128-bit loads where aligned) produces the
+//                            bit-packed mask, the three threshold counts, the stability score and the filtered score.
+//   nms_order_kernel         one CTA: bitonic sort of the (score desc, slot asc) keys in shared memory, valid count.
+//   nms_pairs_kernel         64 x 64 tiles of sorted positions (upper triangle): AND + popc over the bit-packed masks
+//                            staged through shared memory, comparisons turned into 64-bit suppression words by ballots.
+//   nms_scan_kernel          one CTA: greedy walk in blocks of 64; one warp resolves a block against its diagonal
+//                            words, then every thread ORs the kept rows into the "removed" bitset.
+#include <math.h>
+#include "psam_common.cuh"
+#include "../../include/psam_b200.h"
+
+namespace {
+
+constexpr int kCandThreads = 256;
+constexpr int kNmsMaxK = 16384;
+constexpr int kTile = 64;       // sorted positions per tile side / per scan block
+constexpr int kTileWords = 32;  // mask words staged per shared-memory round
+constexpr int kScanThreads = 512;
+
+__device__ __forceinline__ bool candidate_survives(float iou, float stab, int area, float iou_t, float stab_t, int min_area) {
+    if (!(iou == iou)) return false;  // a NaN predicted IoU is never kept
+    if (iou_t > 0.f && !(iou > iou_t)) return false;
+    if (stab_t > 0.f && !(stab >= stab_t)) return false;
+    return area >= min_area && area >= 1;
+}
+
+template <bool VEC>
+__global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const float* __restrict__ logits,
+                                                                       const float* __restrict__ iou_preds, int N,
+                                                                       float thr, float thr_hi, float thr_lo, float iou_t,
+                                                                       float stab_t, int min_area, long long base, int W,
+                                                                       uint32_t* __restrict__ bits, int* __restrict__ area_out,
+                                                                       float* __restrict__ stab_out, float* __restrict__ score_out) {
+    psam::pdl_prologue();
+    constexpr int U = 4;  // warp iterations whose loads are issued together
+    const int row = blockIdx.x;
+    const float* rp = logits + (size_t)row * N;
+    const long long slot = base + row;
+    uint32_t* bp = bits + (size_t)slot * W;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int n_area = 0, n_hi = 0, n_lo = 0;
+    if (VEC) {
+        // a warp iteration covers 128 points = 4 words; lane l holds points 4l..4l+3 of it
+        const float4* rp4 = reinterpret_cast<const float4*>(rp);
+        const int n4 = N >> 2;
+        const int iters = (W + 3) >> 2;
+        for (int it0 = warp * U; it0 < iters; it0 += nw * U) {
+            float4 v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int q = (it0 + u) * 32 + lane;
+                v[u] = q < n4 ? __ldcs(rp4 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int it = it0 + u;
+                if (it >= iters) break;  // warp-uniform
+                const bool in = it * 32 + lane < n4;
+                const float x[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+                uint32_t nib = 0;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    if (in) {
+                        nib |= (uint32_t)(x[e] > thr) << e;
+                        n_hi += x[e] > thr_hi;
+                        n_lo += x[e] > thr_lo;
+                    }
+                }
+                n_area += __popc(nib);
+                uint32_t word = nib << (4 * (lane & 7));
+                word |= __shfl_xor_sync(0xffffffffu, word, 1);
+                word |= __shfl_xor_sync(0xffffffffu, word, 2);
+                word |= __shfl_xor_sync(0xffffffffu, word, 4);
+                const int w = it * 4 + (lane >> 3);
+                if ((lane & 7) == 0 && w < W) bp[w] = word;
+            }
+        }
+    } else {
+        // a warp iteration covers 32 points = one word, built by a ballot
+        for (int it0 = warp * U; it0 < W; it0 += nw * U) {
+            float v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int p = (it0 + u) * 32 + lane;
+                v[u] = p < N ? __ldcs(rp + p) : 0.f;
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int it = it0 + u;
+                if (it >= W) break;  // warp-uniform
+                const bool in = it * 32 + lane < N;
+                const bool b = in && v[u] > thr;
+                n_hi += in && v[u] > thr_hi;
+                n_lo += in && v[u] > thr_lo;
+                const uint32_t word = __ballot_sync(0xffffffffu, b);
+                n_area += b;
+                if (lane == 0) bp[it] = word;
+            }
+        }
+    }
+    __shared__ int red[3][kCandThreads / 32];
+    n_area = __reduce_add_sync(0xffffffffu, n_area);
+    n_hi = __reduce_add_sync(0xffffffffu, n_hi);
+    n_lo = __reduce_add_sync(0xffffffffu, n_lo);
+    if (lane == 0) {
+        red[0][warp] = n_area;
+        red[1][warp] = n_hi;
+        red[2][warp] = n_lo;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int a = 0, h = 0, l = 0;
+        for (int i = 0; i < nw; ++i) {
+            a += red[0][i];
+            h += red[1][i];
+            l += red[2][i];
+        }
+        const float stab = __fdiv_rn(__int2float_rn(h), __int2float_rn(l));
+        const float iou = iou_preds[row];
+        area_out[slot] = a;
+        stab_out[slot] = stab;
+        score_out[slot] = candidate_survives(iou, stab, a, iou_t, stab_t, min_area) ? iou : -INFINITY;
+    }
+}
+
+// ---- NMS a: order ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(1024) nms_order_kernel(const float* __restrict__ score, int K, int P2, int* __restrict__ order,
+                                                         int* __restrict__ count) {
+    psam::pdl_prologue();
+    extern __shared__ unsigned long long keys[];
+    __shared__ int n_valid;
+    if (threadIdx.x == 0) n_valid = 0;
+    __syncthreads();
+    int valid = 0;
+    for (int i = threadIdx.x; i < P2; i += blockDim.x) {
+        unsigned long long k = ~0ull;  // dropped and padding entries sort last
+        if (i < K) {
+            const float s = score[i];
+            if (s > -INFINITY) {  // -inf (filtered) and NaN are dropped
+                uint32_t u = __float_as_uint(s);
+                u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);  // monotone in s
+                k = ((unsigned long long)(~u) << 32) | (uint32_t)i;  // ascending key = score descending, slot ascending
+                ++valid;
+            }
+        }
+        keys[i] = k;
+    }
+    if (valid) atomicAdd(&n_valid, valid);
+    for (int k = 2; k <= P2; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            __syncthreads();
+            for (int p = threadIdx.x; p < (P2 >> 1); p += blockDim.x) {
+                const int i = ((p & ~(j - 1)) << 1) | (p & (j - 1));
+                const int l = i + j;
+                const bool up = (i & k) == 0;
+                const unsigned long long a = keys[i], b = keys[l];
+                if ((a > b) == up) {
+                    keys[i] = b;
+                    keys[l] = a;
+                }
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < K; i += blockDim.x) order[i] = (int)(uint32_t)(keys[i] & 0xffffffffull);
+    if (threadIdx.x == 0) *count = n_valid;
+}
+
+// ---- NMS b: pairwise suppression bits ---------------------------------------------------------------------------
+// Tile (bi, bj), bj >= bi, of sorted positions.  Thread (ty, tx) of 16 x 16 owns rows ty*4 + r and columns tx + 16 c.
+__global__ void __launch_bounds__(256) nms_pairs_kernel(const uint32_t* __restrict__ bits, const int* __restrict__ area, int W,
+                                                        float nms_thresh, const int* __restrict__ order,
+                                                        const int* __restrict__ count_p, unsigned long long* __restrict__ mat,
+                                                        int ldm) {
+    psam::pdl_prologue();
+    const int bi = blockIdx.y, bj = blockIdx.x;
+    if (bj < bi) return;
+    const int count = *count_p;
+    if (bj * kTile >= count) return;  // beyond the valid candidates (bi <= bj)
+    __shared__ __align__(16) uint32_t sa[kTileWords][kTile];
+    __shared__ __align__(16) uint32_t sb[kTileWords][kTile];
+    __shared__ int slot_a[kTile], slot_b[kTile], area_a[kTile], area_b[kTile];
+    const int tid = threadIdx.x;
+    if (tid < 2 * kTile) {
+        const int r = tid & (kTile - 1);
+        const int pos = (tid < kTile ? bi : bj) * kTile + r;
+        const int s = pos < count ? order[pos] : -1;
+        const int a = s >= 0 ? area[s] : 0;
+        if (tid < kTile) {
+            slot_a[r] = s;
+            area_a[r] = a;
+        } else {
+            slot_b[r] = s;
+            area_b[r] = a;
+        }
+    }
+    __syncthreads();
+    const int tx = tid & 15, ty = tid >> 4;
+    uint32_t acc[4][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) acc[r][c] = 0;
+    for (int w0 = 0; w0 < W; w0 += kTileWords) {
+        const int kw = min(kTileWords, W - w0);
+        for (int e = tid; e < kTileWords * kTile; e += blockDim.x) {
+            const int r = e & (kTile - 1), w = e >> 6;
+            const int ga = slot_a[r], gb = slot_b[r];
+            const bool inw = w < kw;
+            sa[w][r] = (ga >= 0 && inw) ? bits[(size_t)ga * W + w0 + w] : 0u;
+            sb[w][r] = (gb >= 0 && inw) ? bits[(size_t)gb * W + w0 + w] : 0u;
+        }
+        __syncthreads();
+#pragma unroll 4
+        for (int w = 0; w < kw; ++w) {
+            const uint4 a4 = *reinterpret_cast<const uint4*>(&sa[w][ty * 4]);
+            const uint32_t a[4] = {a4.x, a4.y, a4.z, a4.w};
+            const uint32_t b[4] = {sb[w][tx], sb[w][tx + 16], sb[w][tx + 32], sb[w][tx + 48]};
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[r][c] += __popc(a[r] & b[c]);
+        }
+        __syncthreads();
+    }
+    // epilogue: one ballot per (r, c); the half-warp of each ty contributes 16 columns
+    const int half = (tid >> 4) & 1;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int li = ty * 4 + r;
+        const int gi = bi * kTile + li;
+        unsigned long long word = 0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int lj = tx + 16 * c;
+            const int gj = bj * kTile + lj;
+            bool sup = false;
+            if (gi < count && gj < count && gj > gi) {
+                const int inter = (int)acc[r][c];
+                const int uni = area_a[li] + area_b[lj] - inter;
+                sup = __fdiv_rn(__int2float_rn(inter), __int2float_rn(uni)) > nms_thresh;
+            }
+            const uint32_t bal = __ballot_sync(0xffffffffu, sup);
+            word |= (unsigned long long)((bal >> (16 * half)) & 0xffffu) << (16 * c);
+        }
+        if (tx == 0 && gi < count) mat[(size_t)gi * ldm + bj] = word;
+    }
+}
+
+// ---- NMS c: greedy scan ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const unsigned long long* __restrict__ mat, int ldm,
+                                                                const int* __restrict__ order, const int* __restrict__ count_p,
+                                                                int* __restrict__ keep, int* __restrict__ keep_count) {
+    psam::pdl_prologue();
+    __shared__ unsigned long long removed[kNmsMaxK / kTile];
+    __shared__ int kept_rows[kTile];
+    __shared__ int n_block, n_kept;
+    const int count = *count_p;
+    const int nb = (count + kTile - 1) / kTile;
+    const int tid = threadIdx.x;
+    for (int c = tid; c < nb; c += blockDim.x) removed[c] = 0ull;
+    if (tid == 0) n_kept = 0;
+    __syncthreads();
+    for (int b = 0; b < nb; ++b) {
+        if (tid < 32) {
+            const int lane = tid;
+            const int rows = min(kTile, count - b * kTile);
+            const size_t r0 = (size_t)b * kTile;
+            const unsigned long long d0 = lane < rows ? mat[(r0 + lane) * ldm + b] : 0ull;
+            const unsigned long long d1 = lane + 32 < rows ? mat[(r0 + lane + 32) * ldm + b] : 0ull;
+            unsigned long long rem = removed[b], km = 0ull;
+            for (int i = 0; i < rows; ++i) {
+                const unsigned long long di = __shfl_sync(0xffffffffu, i < 32 ? d0 : d1, i & 31);
+                if (!((rem >> i) & 1ull)) {
+                    km |= 1ull << i;
+                    rem |= di;
+                }
+            }
+            const int base = n_kept;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int pos = lane + 32 * h;
+                if ((km >> pos) & 1ull) {
+                    const int rank = __popcll(km & ((1ull << pos) - 1ull));
+                    keep[base + rank] = order[r0 + pos];
+                    kept_rows[rank] = pos;
+                }
+            }
+            __syncwarp();
+            if (lane == 0) {
+                n_block = __popcll(km);
+                n_kept = base + n_block;
+            }
+        }
+        __syncthreads();
+        const int ncols = nb - b - 1;
+        const int total = n_block * ncols;
+        for (int e = tid; e < total; e += blockDim.x) {
+            const int r = e / ncols, c = b + 1 + e % ncols;
+            const unsigned long long v = mat[((size_t)b * kTile + kept_rows[r]) * ldm + c];
+            if (v) atomicOr(&removed[c], v);
+        }
+        __syncthreads();
+    }
+    if (tid == 0) *keep_count = n_kept;
+}
+
+size_t nms_order_bytes(int K) { return ((size_t)K * sizeof(int) + 15) / 16 * 16; }
+
+}  // namespace
+
+extern "C" int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z, int C, int N, float mask_threshold,
+                                        float stability_offset, float pred_iou_thresh, float stability_thresh, int min_area,
+                                        long long base, int W, uint32_t* bits, int* area, float* stability, float* score,
+                                        cudaStream_t stream) {
+    if (!logits || !iou_preds || !bits || !area || !stability || !score) return PSAM_ERR_ARG;
+    if (Z <= 0 || C <= 0 || N <= 0 || base < 0 || W < psam::ceil_div(N, 32)) return PSAM_ERR_ARG;
+    if ((long long)Z * C > 0x7fffffffLL) return PSAM_ERR_ARG;
+    const float thr_hi = mask_threshold + stability_offset, thr_lo = mask_threshold - stability_offset;
+    const bool vec = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(logits) % 16 == 0);
+    auto kernel = vec ? mask_candidates_kernel<true> : mask_candidates_kernel<false>;
+    PSAM_CUDA_TRY(psam::launch(kernel, dim3(Z * C), dim3(kCandThreads), (size_t)0, stream, logits, iou_preds, N, mask_threshold,
+                               thr_hi, thr_lo, pred_iou_thresh, stability_thresh, min_area, base, W, bits, area, stability,
+                               score));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" size_t psam_mask_nms_workspace_bytes(int K, int W) {
+    (void)W;
+    if (K < 0 || K > kNmsMaxK) return 0;
+    const size_t ldm = (size_t)(K + kTile - 1) / kTile;
+    return 16 + nms_order_bytes(K) + (size_t)K * ldm * sizeof(unsigned long long);
+}
+
+extern "C" int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh,
+                             int* keep, int* keep_count, void* workspace, cudaStream_t stream) {
+    if (!keep || !keep_count || !workspace || K < 0 || K > kNmsMaxK) return PSAM_ERR_ARG;
+    if (K > 0 && (!bits || !area || !score || W <= 0)) return PSAM_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
+    char* ws = static_cast<char*>(workspace);
+    int* count = reinterpret_cast<int*>(ws);
+    int* order = reinterpret_cast<int*>(ws + 16);
+    auto* mat = reinterpret_cast<unsigned long long*>(ws + 16 + nms_order_bytes(K));
+    const int ldm = (K + kTile - 1) / kTile;
+    int P2 = 2;
+    while (P2 < K) P2 <<= 1;
+    const size_t smem = (size_t)P2 * sizeof(unsigned long long);
+    if (smem > 48 * 1024)
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(nms_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PSAM_CUDA_TRY(psam::launch(nms_order_kernel, dim3(1), dim3(1024), smem, stream, score, K, P2, order, count));
+    PSAM_LAUNCH_CHECK();
+    if (K > 0) {
+        PSAM_CUDA_TRY(psam::launch(nms_pairs_kernel, dim3(ldm, ldm), dim3(256), (size_t)0, stream, bits, area, W, nms_thresh,
+                                   (const int*)order, (const int*)count, mat, ldm));
+        PSAM_LAUNCH_CHECK();
+    }
+    PSAM_CUDA_TRY(psam::launch(nms_scan_kernel, dim3(1), dim3(kScanThreads), (size_t)0, stream, (const unsigned long long*)mat,
+                               ldm, (const int*)order, (const int*)count, keep, keep_count));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}

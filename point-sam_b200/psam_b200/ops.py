@@ -329,3 +329,54 @@ def split_f32(x: torch.Tensor, out: Split, add: Optional[torch.Tensor] = None):
         nv.check(nv.lib().psam_split_add_f32(nv.ptr(x), nv.ptr(add), x.shape[-1], rows, x.shape[-1], out.ptr(), out.plane, out.pitch,
                                              out.pitch, nv.stream()), "split_add_f32")
 
+
+
+# ------------------------------------------------------------------------------------------------
+# automatic mask generation: candidate extraction and mask NMS
+# ------------------------------------------------------------------------------------------------
+NMS_MAX_CANDIDATES = 16384
+
+
+def mask_words(N: int) -> int:
+    """32-bit words of one bit-packed mask of N points."""
+    return (N + 31) // 32
+
+
+def mask_candidates(logits: torch.Tensor, iou_preds: torch.Tensor, *, mask_threshold: float = 0.0,
+                    stability_offset: float = 1.0, pred_iou_thresh: float = 0.0, stability_thresh: float = 0.0,
+                    min_area: int = 0, out=None, base: int = 0):
+    """Candidate extraction (psam_mask_candidates_f32): logits [Z,C,N], iou_preds [Z,C] fill slots base .. base + Z*C of
+    out = (bits [K,W] int32 bit patterns, area [K] int32, stability [K] fp32, score [K] fp32; -inf = filtered out).
+    Without `out` the four tensors are allocated for K = Z*C slots."""
+    Z, C, N = logits.shape
+    lg = logits.float().contiguous()
+    io = iou_preds.float().contiguous()
+    if out is None:
+        if base != 0:
+            raise ValueError("mask_candidates: base needs a caller-owned `out`")
+        K, dev = Z * C, logits.device
+        out = (torch.empty((K, mask_words(N)), dtype=torch.int32, device=dev), torch.empty(K, dtype=torch.int32, device=dev),
+               torch.empty(K, dtype=torch.float32, device=dev), torch.empty(K, dtype=torch.float32, device=dev))
+    bits, area, stab, score = out
+    if base < 0 or base + Z * C > bits.shape[0]:
+        raise ValueError(f"mask_candidates: slots {base}..{base + Z * C} do not fit {bits.shape[0]} candidates")
+    nv.check(nv.lib().psam_mask_candidates_f32(nv.ptr(lg), nv.ptr(io), Z, C, N, float(mask_threshold), float(stability_offset),
+                                               float(pred_iou_thresh), float(stability_thresh), int(min_area), int(base),
+                                               bits.shape[1], nv.ptr(bits), nv.ptr(area), nv.ptr(stab), nv.ptr(score),
+                                               nv.stream()), "mask_candidates")
+    return out
+
+
+def mask_nms(bits: torch.Tensor, area: torch.Tensor, score: torch.Tensor, nms_thresh: float):
+    """Greedy mask-IoU NMS (psam_mask_nms) over the K candidates of mask_candidates.  Returns (keep [max(K,1)] int32, the
+    kept candidate indices in score order, and keep_count [1] int32); both stay on the device."""
+    K, W = bits.shape
+    if K > NMS_MAX_CANDIDATES:
+        raise ValueError(f"mask_nms: {K} candidates, at most {NMS_MAX_CANDIDATES}")
+    dev = bits.device
+    keep = torch.empty(max(K, 1), dtype=torch.int32, device=dev)
+    keep_count = torch.empty(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(nv.lib().psam_mask_nms_workspace_bytes(K, W), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_mask_nms(nv.ptr(bits) if K else None, nv.ptr(area) if K else None, nv.ptr(score) if K else None, K, W,
+                                    float(nms_thresh), nv.ptr(keep), nv.ptr(keep_count), nv.ptr(ws), nv.stream()), "mask_nms")
+    return keep, keep_count
