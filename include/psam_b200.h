@@ -335,6 +335,32 @@ size_t psam_mask_nms_workspace_bytes(int K, int W);
 int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh, int* keep,
                   int* keep_count, void* workspace, cudaStream_t stream);
 
+/* Small-region post-processing of the kept masks: segment-anything's SamAutomaticMaskGenerator.postprocess_small_regions /
+ * remove_small_regions (min_mask_region_area), restated for a point cloud of N points.
+ * Connectivity: nbr [N, k1] int64 is the cloud's kNN graph (psam_knn_f32(xyz, xyz, k1); the generator uses
+ * k1 = min(9, N), the analogue of 8-connectivity).  {i, j} is an edge when j = nbr[i, t] for some t and i != j (undirected);
+ * an entry outside 0..N-1 is no edge.  Only edges with both ends in the working set count (the induced subgraph).
+ * For every kept rank p < *keep_count (read on the device), on the mask m = bits[keep[p]]:
+ *   1. holes:   working set = the points n < N outside m; every component of fewer than min_area points joins m.
+ *               changed_h = at least one did.
+ *   2. islands: working set = m (after step 1).  If some component has fewer than min_area points (changed_i), m keeps
+ *               its components of >= min_area points, or, when none reaches min_area, only the largest one (on equal
+ *               sizes the one whose smallest point index is lowest).
+ * Outputs by rank p (so they feed psam_mask_nms directly): bits_out[p*W .. p*W+W) the new mask (bits past N and words past
+ * ceil(N/32) zero), area_out[p] its point count, score_out[p] = 1 if neither step changed the mask, 0 otherwise (SAM's
+ * rescoring); ranks p >= *keep_count get score_out[p] = -inf and nothing else.  A non-empty mask stays non-empty.
+ * The result is exact and independent of scheduling: every decision is made on exact integer counts of unique components.
+ * bits [K', W] (W >= ceil(N/32)) and keep [K] are the outputs of psam_mask_candidates_f32 / psam_mask_nms, K <= 16384,
+ * 1 <= N <= 1048576, 1 <= k1 <= N, min_area >= 1.  bits / keep / outputs may be NULL when K == 0.
+ * workspace: psam_mask_regions_workspace_bytes(K, N) bytes, 16-byte aligned.  Labels of up to 49152 points live in shared
+ * memory (16 bytes); beyond that the workspace holds one 4N-byte label slice per CTA, min(K, 132, 24 MiB / 4N) slices
+ * (at least one), rounded up to 16 bytes.
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_mask_regions_workspace_bytes(int K, int N);
+int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep, const int* keep_count, const long long* nbr,
+                      int k1, int min_area, uint32_t* bits_out, int* area_out, float* score_out, void* workspace,
+                      cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

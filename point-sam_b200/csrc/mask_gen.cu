@@ -8,6 +8,9 @@
 //                            staged through shared memory, comparisons turned into 64-bit suppression words by ballots.
 //   nms_scan_kernel          one CTA: greedy walk in blocks of 64; one warp resolves a block against its diagonal
 //                            words, then every thread ORs the kept rows into the "removed" bitset.
+//   mask_regions_kernel<S>   one CTA per kept mask: lock-free union-find over the kNN graph, first on the points outside
+//                            the mask (small holes are filled), then on the mask (small islands are removed); labels in
+//                            shared memory (S = true, N <= 49152) or in a per-CTA slice of the workspace.
 #include <math.h>
 #include "psam_common.cuh"
 #include "../../include/psam_b200.h"
@@ -310,6 +313,175 @@ __global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const unsigned l
 
 size_t nms_order_bytes(int K) { return ((size_t)K * sizeof(int) + 15) / 16 * 16; }
 
+// ---- small-region post-processing: connected components over the kNN graph ------------------------------------------
+// One CTA per kept mask (persistent over the ranks).  par[] is a union-find forest over the points of the working set with
+// par[i] <= i at all times, so every root is the smallest point of its component and the forest's final shape does not
+// depend on the order in which edges are hooked.  After flattening, a root's entry holds -(component size).
+constexpr int kRegionThreads = 1024;
+constexpr int kRegionSmemMaxN = 49152;        // 4 B of labels + 1 bit of mask per point in shared memory
+constexpr int kRegionMaxN = 1 << 20;           // the mask words (N / 8 bytes) always stay in shared memory: 128 KB
+constexpr long long kRegionL2Bytes = 24ll << 20;  // workspace form: label slices meant to stay L2-resident
+constexpr int kRegionMaxSlices = 132;
+
+// label slices of the workspace form (one per CTA): as many as fit kRegionL2Bytes, at most kRegionMaxSlices and K
+int region_slices(int K, int N) {
+    long long fit = kRegionL2Bytes / ((long long)N * 4);
+    fit = fit < 1 ? 1 : (fit > kRegionMaxSlices ? kRegionMaxSlices : fit);
+    return K < fit ? K : (int)fit;
+}
+
+__device__ __forceinline__ bool region_member(const uint32_t* sw, int i, int N, bool invert) {
+    return i < N && (((sw[i >> 5] >> (i & 31)) & 1u) != (uint32_t)invert);
+}
+
+// root of i with path halving (ECL-CC), used while edges are hooked.  A stale halving store still writes an ancestor,
+// which is all the hooking needs.  The flatten pass does not use it (see there).
+__device__ __forceinline__ int region_find(volatile int* par, int i) {
+    int cur = par[i];
+    if (cur != i) {
+        int prev = i, next;
+        while (cur > (next = par[cur])) {
+            par[prev] = next;
+            prev = cur;
+            cur = next;
+        }
+    }
+    return cur;
+}
+
+// Labels the components of {i < N : bit i of sw != invert} under the edges {i, nbr[i*k1 + t]}.  On return, for a member i:
+// par[i] < 0 -> i is a root of a component of -par[i] points; otherwise par[i] is its root.
+__device__ void region_components(const uint32_t* sw, bool invert, int N, const long long* __restrict__ nbr, int k1, int* par) {
+    volatile int* vp = par;
+    for (int i = threadIdx.x; i < N; i += blockDim.x) par[i] = i;
+    __syncthreads();
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+        if (!region_member(sw, i, N, invert)) continue;
+        const long long* row = nbr + (size_t)i * k1;
+        for (int t = 0; t < k1; ++t) {
+            const long long jj = row[t];
+            if (jj < 0 || jj >= N || jj == i) continue;  // an index outside the cloud is no edge
+            const int j = (int)jj;
+            if (!region_member(sw, j, N, invert)) continue;
+            int a = region_find(vp, i), b = region_find(vp, j);
+            while (a != b) {  // hook the larger root under the smaller one; on a lost race climb to the winner
+                if (a < b) {
+                    const int r = atomicCAS(par + b, b, a);
+                    if (r == b) break;
+                    b = r;
+                } else {
+                    const int r = atomicCAS(par + a, a, b);
+                    if (r == a) break;
+                    a = r;
+                }
+            }
+        }
+    }
+    __syncthreads();
+    // flatten: a read-only walk, and each thread writes only its own entry.  Path halving here could let a stale store
+    // re-point an entry that another thread has already set to its root.  Every concurrent write replaces an ancestor by
+    // the root, so each walk still ends at the root.
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+        if (!region_member(sw, i, N, invert)) continue;
+        int r = vp[i], n;
+        while (r > (n = vp[r])) r = n;
+        vp[i] = r;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < N; i += blockDim.x)
+        if (par[i] == i && region_member(sw, i, N, invert)) par[i] = -1;
+    __syncthreads();
+    for (int i = threadIdx.x; i < N; i += blockDim.x) {
+        const int r = par[i];
+        if (r >= 0 && r != i && region_member(sw, i, N, invert)) atomicSub(par + r, 1);
+    }
+    __syncthreads();
+}
+
+__device__ __forceinline__ int region_root(const int* par, int i) { return par[i] < 0 ? i : par[i]; }
+
+template <bool SMEM>
+__global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint32_t* __restrict__ bits, int K, int W, int N,
+                                                                      const int* __restrict__ keep, const int* __restrict__ keep_count,
+                                                                      const long long* __restrict__ nbr, int k1, int min_area,
+                                                                      uint32_t* __restrict__ bits_out, int* __restrict__ area_out,
+                                                                      float* __restrict__ score_out, int* __restrict__ workspace) {
+    psam::pdl_prologue();
+    extern __shared__ __align__(16) uint32_t region_smem[];
+    const int Wn = (N + 31) >> 5;
+    uint32_t* sw = region_smem;
+    int* par = SMEM ? reinterpret_cast<int*>(region_smem + ((Wn + 3) & ~3)) : workspace + (size_t)blockIdx.x * N;
+    __shared__ int changed, any_small, area_red;
+    __shared__ unsigned long long best;  // (size << 32) | ~root: the largest component, smallest root on equal sizes
+    const int count = *keep_count;
+    const int lane = threadIdx.x & 31;
+    for (int p = blockIdx.x; p < K; p += gridDim.x) {
+        if (p >= count) {
+            if (threadIdx.x == 0) score_out[p] = -INFINITY;
+            continue;
+        }
+        const uint32_t* src = bits + (size_t)keep[p] * W;
+        for (int w = threadIdx.x; w < Wn; w += blockDim.x) {
+            const int tail = N - 32 * w;
+            sw[w] = tail >= 32 ? src[w] : src[w] & ((1u << tail) - 1u);
+        }
+        if (threadIdx.x == 0) {
+            changed = 0;
+            any_small = 0;
+            area_red = 0;
+            best = 0ull;
+        }
+        __syncthreads();
+        // 1. holes: components of the complement smaller than min_area join the mask
+        region_components(sw, true, N, nbr, k1, par);
+        for (int i = threadIdx.x; i < Wn * 32; i += blockDim.x) {  // a warp owns whole words
+            const uint32_t word = sw[i >> 5];
+            const bool in = (word >> (i & 31)) & 1u;
+            const bool fill = !in && i < N && -par[region_root(par, i)] < min_area;
+            const uint32_t add = __ballot_sync(0xffffffffu, fill);
+            if (lane == 0 && add) {
+                sw[i >> 5] = word | add;
+                changed = 1;
+            }
+        }
+        __syncthreads();
+        // 2. islands: components of the mask smaller than min_area leave it; if none reaches min_area, the largest stays
+        region_components(sw, false, N, nbr, k1, par);
+        for (int i = threadIdx.x; i < N; i += blockDim.x) {
+            if (par[i] < 0 && region_member(sw, i, N, false)) {
+                const int size = -par[i];
+                if (size < min_area) any_small = 1;
+                atomicMax(&best, ((unsigned long long)size << 32) | (uint32_t)~i);
+            }
+        }
+        __syncthreads();
+        const bool drop = any_small != 0;
+        const int keep_root = (int)~(uint32_t)(best & 0xffffffffull);
+        const bool none_big = (int)(best >> 32) < min_area;
+        int a = 0;
+        for (int i = threadIdx.x; i < Wn * 32; i += blockDim.x) {
+            const uint32_t word = sw[i >> 5];
+            bool in = (word >> (i & 31)) & 1u;
+            if (drop && in) {
+                const int r = region_root(par, i);
+                in = none_big ? r == keep_root : -par[r] >= min_area;
+            }
+            const uint32_t out = __ballot_sync(0xffffffffu, in);
+            if (lane == 0) bits_out[(size_t)p * W + (i >> 5)] = out;
+            a += in;
+        }
+        for (int w = Wn + threadIdx.x; w < W; w += blockDim.x) bits_out[(size_t)p * W + w] = 0u;
+        a = __reduce_add_sync(0xffffffffu, a);
+        if (lane == 0 && a) atomicAdd(&area_red, a);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            area_out[p] = area_red;
+            score_out[p] = (changed || drop) ? 0.f : 1.f;
+        }
+        __syncthreads();  // sw, par and the shared flags are reused by the next rank
+    }
+}
+
 }  // namespace
 
 extern "C" int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z, int C, int N, float mask_threshold,
@@ -360,6 +532,42 @@ extern "C" int psam_mask_nms(const uint32_t* bits, const int* area, const float*
     }
     PSAM_CUDA_TRY(psam::launch(nms_scan_kernel, dim3(1), dim3(kScanThreads), (size_t)0, stream, (const unsigned long long*)mat,
                                ldm, (const int*)order, (const int*)count, keep, keep_count));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" size_t psam_mask_regions_workspace_bytes(int K, int N) {
+    if (K < 0 || K > kNmsMaxK || N <= 0 || N > kRegionMaxN) return 0;
+    if (N <= kRegionSmemMaxN) return 16;
+    const size_t bytes = ((size_t)region_slices(K, N) * N * sizeof(int) + 15) / 16 * 16;
+    return bytes < 16 ? 16 : bytes;
+}
+
+extern "C" int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep, const int* keep_count,
+                                 const long long* nbr, int k1, int min_area, uint32_t* bits_out, int* area_out, float* score_out,
+                                 void* workspace, cudaStream_t stream) {
+    if (!keep_count || !nbr || !workspace) return PSAM_ERR_ARG;
+    if (K > 0 && (!bits || !keep || !bits_out || !area_out || !score_out)) return PSAM_ERR_ARG;
+    if (N <= 0 || N > kRegionMaxN || W < psam::ceil_div(N, 32) || k1 < 1 || k1 > N || K < 0 || K > kNmsMaxK || min_area < 1)
+        return PSAM_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
+    if (K == 0) return PSAM_OK;
+    // persistent grid: two CTAs per SM in the shared-memory form, one per label slice (at most one per SM) otherwise
+    int dev = 0, sms = 0;
+    PSAM_CUDA_TRY(cudaGetDevice(&dev));
+    PSAM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int grid = N <= kRegionSmemMaxN ? min(K, 2 * sms) : min(region_slices(K, N), sms);
+    const size_t words = (size_t)(psam::ceil_div(N, 32) + 3) / 4 * 4 * sizeof(uint32_t);
+    if (N <= kRegionSmemMaxN) {
+        const size_t smem = words + (size_t)N * sizeof(int);
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<true>, dim3(grid), dim3(kRegionThreads), smem, stream, bits, K, W, N, keep,
+                                   keep_count, nbr, k1, min_area, bits_out, area_out, score_out, (int*)nullptr));
+    } else {
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)words));
+        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<false>, dim3(grid), dim3(kRegionThreads), words, stream, bits, K, W, N, keep,
+                                   keep_count, nbr, k1, min_area, bits_out, area_out, score_out, static_cast<int*>(workspace)));
+    }
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }

@@ -9,6 +9,9 @@
 4. After each batch, ``psam_mask_candidates_f32`` bit-packs the masks, computes areas and stability scores and applies
    the predicted-IoU / stability / area filters.
 5. ``psam_mask_nms`` removes duplicates by greedy mask-IoU NMS over all candidates of the cloud.
+6. With ``min_mask_region_area > 0`` (SAM's post-processing): ``psam_knn_f32`` builds the cloud's kNN graph,
+   ``psam_mask_regions`` fills small holes of every kept mask and removes its small islands (connected components of that
+   graph), rescores the masks (1 unchanged, 0 changed) and ``psam_mask_nms`` runs again on the result.
 
 Everything runs on the GPU, and the only host synchronisation is the final read of the number of kept masks.  The
 default thresholds are SAM's; they are not tuned for Point-SAM.
@@ -39,9 +42,13 @@ class PointCloudMaskGenerator:
       stability_score_offset  logit offset of the stability score: count(logit > +off) / count(logit > -off)
       mask_nms_thresh         drop a mask whose IoU with a higher-scoring kept mask is > this
       min_mask_area           keep masks of at least this many points (an empty mask is never kept)
+    generate / generate_packed take SAM's min_mask_region_area as a keyword (default 0: off).
     The model must be in eval mode.  The candidate count points_per_cloud * 3 is limited to 16384."""
 
     mask_threshold = 0.0  # a point is in the mask when its logit is > 0 (as in predict_masks' callers)
+    # neighbours per point of the kNN graph that defines connectivity for min_mask_region_area (the analogue of SAM's
+    # 8-connected pixel grid); the graph is undirected, so a point's degree can be higher
+    region_neighbors = 8
 
     def __init__(self, model, points_per_cloud: int = 1024, points_per_batch: int = 64, pred_iou_thresh: float = 0.88,
                  stability_score_thresh: float = 0.95, stability_score_offset: float = 1.0, mask_nms_thresh: float = 0.7,
@@ -68,8 +75,11 @@ class PointCloudMaskGenerator:
             raise ValueError(f"{name} must be [N, 3] or [1, N, 3] (one cloud per call), got {tuple(t.shape)}")
         return t.float().contiguous()
 
-    def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor) -> Dict[str, torch.Tensor]:
+    def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
         """Enqueue the whole generation on the current stream; nothing here waits for the device."""
+        if min_mask_region_area < 0:
+            raise ValueError(f"min_mask_region_area must be >= 0, got {min_mask_region_area}")
+        region_area = int(min_mask_region_area)
         m = self.model
         if m.training:
             raise NotImplementedError("psam_b200 is an inference-only path: call model.eval() before generating masks")
@@ -98,36 +108,58 @@ class PointCloudMaskGenerator:
                                     base=s * C)
             bits, area, stab, score = cand
             keep, keep_count = ops.mask_nms(bits, area, score, self.mask_nms_thresh)
-        return dict(bits=bits, area=area, stability=stab, score=score, keep=keep, keep_count=keep_count,
-                    point_index=point_index[0], centers=centers[0], slots=C, device=dev)
+            st = dict(bits=bits, area=area, stability=stab, score=score, keep=keep, keep_count=keep_count,
+                      point_index=point_index[0], centers=centers[0], slots=C, device=dev)
+            if region_area > 0:
+                nbr, _ = ops.knn(xyz, xyz, min(self.region_neighbors + 1, N))
+                rbits, rarea, rscore = ops.mask_regions(bits, keep, keep_count, nbr, region_area)
+                rkeep, rcount = ops.mask_nms(rbits, rarea, rscore, self.mask_nms_thresh)
+                st.update(region_bits=rbits, region_area=rarea, region_score=rscore, region_keep=rkeep, region_count=rcount)
+        return st
 
     @staticmethod
     def _finish(st: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
         """The single host synchronisation: read the kept count together with the out-of-range flag of the prompt
-        encoder, then select the kept candidates (on the device)."""
+        encoder, then select the kept candidates (on the device).  After the small-region stage the count is the second
+        NMS's, its keep list holds ranks of the first, and bits / area come from the post-processed masks."""
         flag = engine.bad_flag(st["device"])
-        n, bad = (int(v) for v in torch.cat([st["keep_count"], flag]).tolist())
+        regions = "region_keep" in st
+        n, bad = (int(v) for v in torch.cat([st["region_count" if regions else "keep_count"], flag]).tolist())
         if bad:
             flag.zero_()
             raise ValueError("Input coordinates must be normalized to [-1, 1].")
-        sel = st["keep"][:n].long()
+        if regions:
+            rank = st["region_keep"][:n].long()
+            sel = st["keep"][rank].long()
+            bits, area = st["region_bits"][rank], st["region_area"][rank]
+        else:
+            sel = st["keep"][:n].long()
+            bits, area = st["bits"][sel], st["area"][sel]
         z = torch.div(sel, st["slots"], rounding_mode="floor")
-        return dict(bits=st["bits"][sel], area=st["area"][sel], predicted_iou=st["score"][sel],
+        return dict(bits=bits, area=area, predicted_iou=st["score"][sel],
                     stability_score=st["stability"][sel], point_index=st["point_index"][z], point_coords=st["centers"][z],
                     mask_slot=sel - z * st["slots"])
 
-    def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor) -> Dict[str, torch.Tensor]:
-        """Masks of one cloud as device tensors, in score order (K = number of kept masks, W = ceil(N / 32)):
+    def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
+        """Masks of one cloud as device tensors (K = number of kept masks, W = ceil(N / 32)):
         bits [K, W] int32 (point n is bit n % 32 of word n // 32), area [K] int32, predicted_iou [K], stability_score [K],
         point_index [K] int64 (index of the prompt point in the cloud), point_coords [K, 3], mask_slot [K] (0..2: which
-        of the three multimask outputs).  xyz / rgb: [N, 3] or [1, N, 3] CUDA tensors, xyz normalised to [-1, 1]."""
-        return self._finish(self._enqueue(xyz, rgb))
+        of the three multimask outputs).  xyz / rgb: [N, 3] or [1, N, 3] CUDA tensors, xyz normalised to [-1, 1].
 
-    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor) -> List[Dict]:
-        """SAM's record list, in score order: segmentation (bool [N] numpy), area, predicted_iou, stability_score,
-        point_coords ([[x, y, z]]), point_index."""
+        min_mask_region_area = 0: the masks are in score order (predicted IoU descending).
+        min_mask_region_area = A > 0 (SAM's post-processing; connectivity = the kNN graph with ``region_neighbors``
+        neighbours per point): every kept mask gets its holes of fewer than A points filled and its islands of fewer than
+        A points removed (if no island reaches A, the largest stays), and mask NMS runs again on the results with
+        unchanged masks ranked before changed ones (ties in the first order).  So the order is: unchanged masks, then
+        changed ones, each in score order.  bits and area are the post-processed ones; predicted_iou and
+        stability_score stay the model's."""
+        return self._finish(self._enqueue(xyz, rgb, min_mask_region_area=min_mask_region_area))
+
+    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> List[Dict]:
+        """SAM's record list, in the order of generate_packed: segmentation (bool [N] numpy), area, predicted_iou,
+        stability_score, point_coords ([[x, y, z]]), point_index."""
         N = self._cloud(xyz, "xyz").shape[1]
-        out = {k: v.cpu().numpy() for k, v in self.generate_packed(xyz, rgb).items()}
+        out = {k: v.cpu().numpy() for k, v in self.generate_packed(xyz, rgb, min_mask_region_area=min_mask_region_area).items()}
         seg = np.unpackbits(out["bits"].astype("<i4").view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
         return [dict(segmentation=seg[i], area=int(out["area"][i]), predicted_iou=float(out["predicted_iou"][i]),
                      stability_score=float(out["stability_score"][i]), point_coords=[out["point_coords"][i].tolist()],

@@ -63,6 +63,7 @@ EXPORTS = [
     "psam_group_max", "psam_softmax_split", "psam_transpose_split", "psam_posenc_f32", "psam_attention_f32",
     "psam_decoder_prepare", "psam_interp_ln_gelu", "psam_interp_add_ln_gelu", "psam_mask_dot", "psam_add_bcast_f32", "psam_split_f32", "psam_split_add_f32",
     "psam_mask_candidates_f32", "psam_mask_nms_workspace_bytes", "psam_mask_nms",
+    "psam_mask_regions_workspace_bytes", "psam_mask_regions",
     "psam_version",
 ]
 
@@ -83,6 +84,8 @@ def lib():
         L.psam_border_prompt_workspace_bytes.argtypes = [i, i, i]
         L.psam_mask_nms_workspace_bytes.restype = c_size_t
         L.psam_mask_nms_workspace_bytes.argtypes = [i, i]
+        L.psam_mask_regions_workspace_bytes.restype = c_size_t
+        L.psam_mask_regions_workspace_bytes.argtypes = [i, i]
         sig = {
             "psam_fps_f32": [p, i, i, i, p, p, p, p],
             "psam_knn_f32": [p, p, i, i, i, i, p, p, p],
@@ -114,6 +117,7 @@ def lib():
             "psam_split_add_f32": [p, p, ll, ll, i, p, ll, ll, ll, p],
             "psam_mask_candidates_f32": [p, p, i, i, i, f, f, f, f, i, ll, i, p, p, p, p, p],
             "psam_mask_nms": [p, p, p, i, i, f, p, p, p, p],
+            "psam_mask_regions": [p, i, i, i, p, p, p, i, i, p, p, p, p, p],
         }
         for name, args in sig.items():
             fn = getattr(L, name)

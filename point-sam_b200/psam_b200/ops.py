@@ -380,3 +380,24 @@ def mask_nms(bits: torch.Tensor, area: torch.Tensor, score: torch.Tensor, nms_th
     nv.check(nv.lib().psam_mask_nms(nv.ptr(bits) if K else None, nv.ptr(area) if K else None, nv.ptr(score) if K else None, K, W,
                                     float(nms_thresh), nv.ptr(keep), nv.ptr(keep_count), nv.ptr(ws), nv.stream()), "mask_nms")
     return keep, keep_count
+
+
+def mask_regions(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor, nbr: torch.Tensor, min_area: int):
+    """Small hole / island removal (psam_mask_regions) on the kept masks keep[:keep_count] of mask_candidates' bits, over
+    the kNN graph nbr [N, k1] or [1, N, k1] int64 (knn(xyz, xyz, k1)).  Returns (bits_out [K,W] int32, area_out [K] int32,
+    score_out [K] fp32), indexed by kept rank with K = len(keep): 1.0 = unchanged, 0.0 = changed, -inf past the kept count.
+    The outputs feed mask_nms directly; nothing waits for the device."""
+    K, W = keep.shape[0], bits.shape[1]
+    N, k1 = nbr.shape[-2], nbr.shape[-1]
+    if K > NMS_MAX_CANDIDATES:
+        raise ValueError(f"mask_regions: {K} kept masks, at most {NMS_MAX_CANDIDATES}")
+    nbr = nbr.reshape(N, k1).contiguous()
+    dev = bits.device
+    bits_out = torch.empty((K, W), dtype=torch.int32, device=dev)
+    area_out = torch.empty(K, dtype=torch.int32, device=dev)
+    score_out = torch.empty(K, dtype=torch.float32, device=dev)
+    ws = torch.empty(nv.lib().psam_mask_regions_workspace_bytes(K, N), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_mask_regions(nv.ptr(bits), K, W, N, nv.ptr(keep), nv.ptr(keep_count), nv.ptr(nbr), k1, int(min_area),
+                                        nv.ptr(bits_out), nv.ptr(area_out), nv.ptr(score_out), nv.ptr(ws), nv.stream()),
+             "mask_regions")
+    return bits_out, area_out, score_out

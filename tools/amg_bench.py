@@ -11,7 +11,12 @@ the kernels'.
 The weights are randomly initialised (no checkpoint is available offline), so SAM's default thresholds would reject every
 candidate; by default the IoU and stability filters are off (every non-empty mask reaches NMS, its largest input).
 --sam-thresholds uses SAM's defaults instead.
-usage: python tools/amg_bench.py [--hier] [--steps 10] [--warmup 2] [--sam-thresholds]"""
+
+--min-region-area A (> 0) adds a "regions" object for SAM's small-region post-processing (min_mask_region_area = A): ms
+per cloud of generate_packed with the stage, against the same without it measured alternately in the same run, the kernel
+time of each op of the stage (kNN graph, mask_regions, second NMS; torch.profiler over 10 launches of the op alone on the
+generator's own inputs, separate run), and the changed and kept counts.  With the default 0 the output is unchanged.
+usage: python tools/amg_bench.py [--hier] [--steps 10] [--warmup 2] [--sam-thresholds] [--min-region-area 0]"""
 import argparse
 import json
 import os
@@ -39,6 +44,7 @@ ap.add_argument("--points", type=int, default=32768)
 ap.add_argument("--prompts", type=int, default=1024)
 ap.add_argument("--batch", type=int, default=64)
 ap.add_argument("--sam-thresholds", action="store_true")
+ap.add_argument("--min-region-area", type=int, default=0)
 a = ap.parse_args()
 if not torch.cuda.is_available():
     sys.exit("amg_bench: needs a CUDA device")
@@ -198,4 +204,57 @@ line = {
     "torch_arm_keep_equal": True,
 }
 line["nms_speedup_vs_torch_arm"] = line["torch_arm_ms"]["nms"] / nms_kernels_ms if nms_kernels_ms else None
+
+
+# ---- small-region post-processing: with / without alternately, then its kernels ----------------------------------------
+def regions_report(A):
+    on, off = [], []
+    for _ in range(a.warmup):
+        gen.generate_packed(xyz, rgb, min_mask_region_area=A)
+    torch.cuda.synchronize()
+    for _ in range(a.steps):
+        for area, dst in ((A, on), (0, off)):
+            t0 = time.perf_counter()
+            gen.generate_packed(xyz, rgb, min_mask_region_area=area)
+            dst.append((time.perf_counter() - t0) * 1e3)
+    st = gen._enqueue(xyz, rgb, min_mask_region_area=A)
+    n1, n2 = int(st["keep_count"].item()), int(st["region_count"].item())
+    changed = int((st["region_score"][:n1] == 0).sum().item())  # rescoring: 0 = changed by the stage
+    # kernel times of the stage: each op profiled alone (torch.profiler, separate run) on the generator's own inputs.  The
+    # encoder's tokenizer also launches knn_kernel and the first NMS the nms_* kernels, so profiling the whole call could
+    # not tell the stage's launches apart.
+    k1 = min(gen.region_neighbors + 1, N)
+    nbr = ops.knn(xyz, xyz, k1)[0]
+    stage = {"knn_graph": (lambda: ops.knn(xyz, xyz, k1), ("knn_kernel",)),
+             "mask_regions": (lambda: ops.mask_regions(st["bits"], st["keep"], st["keep_count"], nbr, A), ("mask_regions_kernel",)),
+             "second_nms": (lambda: ops.mask_nms(st["region_bits"], st["region_area"], st["region_score"], gen.mask_nms_thresh),
+                            ("nms_order_kernel", "nms_pairs_kernel", "nms_scan_kernel"))}
+    reps, kernel_ms = 10, {}
+    for name, (fn, tags) in stage.items():
+        fn()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(reps):
+                fn()
+            torch.cuda.synchronize()
+        per = {}
+        for evt in prof.events():
+            if evt.device_type != torch.autograd.DeviceType.CUDA:
+                continue
+            for tag in tags:
+                if tag in evt.name:
+                    per[tag] = per.get(tag, 0.0) + (getattr(evt, "device_time", None) or evt.cuda_time) / 1e3 / reps
+        kernel_ms[name] = {"ms": sum(per.values()), "kernels": per}
+    return {
+        "min_region_area": A,
+        "ms_per_cloud_with": float(np.median(on)), "ms_per_cloud_without": float(np.median(off)),
+        "ms_per_cloud_with_range": [min(on), max(on)], "ms_per_cloud_without_range": [min(off), max(off)],
+        "stage_ms": float(np.median(on) - np.median(off)),
+        "kernel_ms": kernel_ms,
+        "kept_first_nms": n1, "changed": changed, "kept_after_second_nms": n2,
+    }
+
+
+if a.min_region_area > 0:
+    line["regions"] = regions_report(a.min_region_area)
 print(json.dumps(line))
