@@ -361,6 +361,65 @@ int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep
                       int k1, int min_area, uint32_t* bits_out, int* area_out, float* score_out, void* workspace,
                       cudaStream_t stream);
 
+/* ---- crop layers of automatic mask generation (SAM's crop_n_layers) ------------------------------ */
+/* Layout.  Layer 0 is the whole cloud.  Layer i >= 1 splits every axis a of the cloud's axis-aligned bounding box
+ * [lo_a, hi_a] into n = 2^i crops.  Everything is fp32, every operation rounded on its own (no contraction), in this order:
+ *   lo_a = min_n xyz[n, a], hi_a = max_n xyz[n, a]          (exact; NaN coordinates are ignored, and an axis with
+ *                                                              nothing but NaN gives lo_a = +inf, hi_a = -inf)
+ *   L_a  = hi_a - lo_a
+ *   o_a  = ((r * L_a) * 2) / n                                r = overlap_ratio
+ *   s_a  = (L_a + o_a * (n - 1)) / n
+ *   crop j of the axis: [lo_a + j * (s_a - o_a), lo_a + j * (s_a - o_a) + s_a], except that the last crop's upper bound is
+ *   exactly hi_a (layer 0: [lo_a + 0 * (L_a - o_a), hi_a]).
+ * Crops are numbered layer by layer (layer 0 first), and within layer i as (jx * n + jy) * n + jz, so there are
+ * psam_crop_total(n_layers) = sum_{i <= n_layers} 8^i of them.  boxes[t*6 .. t*6+6) = (x0, y0, z0, x1, y1, z1).
+ * Point n is in crop t when x0 <= x <= x1, y0 <= y <= y1 and z0 <= z <= z1 (closed; a NaN coordinate is in no crop).
+ * counts[t] = the number of points in crop t, or -1 when an earlier crop of the same layer has an identical box (a
+ * duplicate; it happens on zero-extent axes).
+ * 1 <= N, 0 <= n_layers <= 3, 0 <= overlap_ratio < 1.  Two launches (one CTA for the box and the layout, then a grid for
+ * the counts).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_crop_total(int n_layers); /* 0 when n_layers is outside 0..3 */
+int psam_crop_layout_f32(const float* xyz, int N, int n_layers, float overlap_ratio, float* boxes, int* counts,
+                         cudaStream_t stream);
+
+/* Crop gather: the crop cloud of crop `crop` (0 <= crop < n_crops) of psam_crop_layout_f32's boxes, whose n_out points
+ * (its count) come out in ascending global index:
+ *   idx_out[k]       the global index of the crop's k-th point (int32),
+ *   xyz_out[k*3+a]   (p_a - c_a) / scale, where c_a = (x0_a + x1_a) * 0.5 is the box midpoint and scale = sqrt(max_k d2_k),
+ *                    d2 = (dx*dx + dy*dy) + dz*dz with dx = p_x - c_x etc.; every coordinate is 0 when scale is 0, and
+ *                    |xyz_out| <= 1 otherwise (IEEE division and square root),
+ *   rgb_out[k*3+a]   rgb unchanged,
+ *   edge[k/32] bit k%32   the point is within m_a = edge_margin * L_a (L_a = x1_a - x0_a of crop 0, the bounding box) of an
+ *                    interior face of the crop: (x0_a != lo_a and p_a - x0_a <= m_a) or (x1_a != hi_a and x1_a - p_a <= m_a)
+ *                    on some axis a; words up to ceil(n_out / 32) are written (bits past n_out zero).
+ * The compaction is stable and the same on every run.  Two launches.  workspace: psam_crop_gather_workspace_bytes(N)
+ * bytes, 16-byte aligned.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_crop_gather_workspace_bytes(int N);
+int psam_crop_gather_f32(const float* xyz, const float* rgb, int N, const float* boxes, int crop, int n_crops, float edge_margin,
+                         int n_out, int* idx_out, float* xyz_out, float* rgb_out, uint32_t* edge, void* workspace,
+                         cudaStream_t stream);
+
+/* Edge filter (SAM's is_box_near_crop_edge, on masks): score[k] = -inf for every candidate k < K whose mask bits[k*W ..)
+ * shares a point with edge[0 .. W) (the crop's edge bitset).  Run between psam_mask_candidates_f32 and psam_mask_nms.
+ * bits / edge / score may be NULL when K == 0.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_crop_edge_filter(const uint32_t* bits, int K, int W, const uint32_t* edge, float* score, cudaStream_t stream);
+
+/* Uncrop: append a crop's kept masks to the global set.  For every kept rank p < *keep_count (read on the device), with
+ * s = keep[p], z = s / slots and d = *offset_in + p < capacity:
+ *   gbits[d*Wg .. d*Wg+Wg)  the mask bits[s*W ..) of the crop's n points lifted to the cloud's N points (local point k is
+ *                           global point idx[k]; every other bit zero),
+ *   garea[d] = area[s], giou[d] = score[s], gstab[d] = stability[s], gprompt[d] = idx[prompt_index[z]] (int64),
+ *   gslot[d] = s - z * slots, gcrop[d] = crop, gscore[d] = layer_score.
+ * *offset_out = *offset_in + *keep_count (offset_out must not alias offset_in: the caller keeps one entry per crop), and
+ * *overflow = 1 when that exceeds capacity; ranks at or past capacity are not written.
+ * 1 <= n <= N, W >= ceil(n/32), Wg >= ceil(N/32), 1 <= capacity <= 16384, K >= 1 = the length of keep.
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_crop_uncrop(const uint32_t* bits, const int* area, const float* score, const float* stability, int K, int W,
+                     const int* keep, const int* keep_count, const int* idx, int n, const long long* prompt_index, int slots,
+                     int crop, float layer_score, int N, int Wg, int capacity, const int* offset_in, int* offset_out,
+                     uint32_t* gbits, int* garea, float* giou, float* gstab, long long* gprompt, int* gslot, int* gcrop,
+                     float* gscore, int* overflow, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

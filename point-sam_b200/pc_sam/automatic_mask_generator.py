@@ -16,18 +16,34 @@
 Everything runs on the GPU, and the only host synchronisation is the final read of the number of kept masks.  The
 default thresholds are SAM's; they are not tuned for Point-SAM.
 
+Crop layers (keyword ``crop_n_layers > 0``, SAM's zoomed crops for large scenes): ``psam_crop_layout_f32`` splits the cloud's
+bounding box into 2^i x 2^i x 2^i overlapping boxes on layer i and counts their points; the host reads the counts once.
+Layer 0 runs steps 1-5 on the cloud as given.  Every other crop with at least as many points as the tokenizer's first-level
+groups (and a box unlike an earlier one of its layer) is gathered and renormalised by ``psam_crop_gather_f32``, runs steps
+1-5 with ``points_per_cloud // crop_n_points_downscale_factor^i`` prompts, and, before its NMS, drops the candidates that
+touch an interior face of the crop (``psam_crop_edge_filter``).  ``psam_crop_uncrop`` lifts every crop's kept masks to the
+whole cloud, and ``psam_mask_nms`` with score = layer and ``crop_nms_thresh`` merges them (smaller crops win).  Step 6
+then runs on the merged set.  The host synchronises twice: the counts, and the final read.
+
 Memory: each batch of Z = points_per_batch prompts decodes Z rows of N points.  The split-bf16 input of the last
 upscaling Linear is Z*N*Du*4 bytes (Du = 256 for PointCloudSAM, 128 for PointCloudSAMHier): about 2 GB at Z = 64,
 N = 32768, Du = 256.  Lower points_per_batch to trade speed for memory.
 """
 from __future__ import annotations
 
-from typing import Dict, List
+from typing import Dict, List, NamedTuple
 
 import numpy as np
 import torch
 
 from psam_b200 import engine, ops
+
+
+class CropArgs(NamedTuple):
+    n_layers: int
+    nms_thresh: float
+    overlap_ratio: float
+    downscale: int
 
 
 class PointCloudMaskGenerator:
@@ -42,13 +58,22 @@ class PointCloudMaskGenerator:
       stability_score_offset  logit offset of the stability score: count(logit > +off) / count(logit > -off)
       mask_nms_thresh         drop a mask whose IoU with a higher-scoring kept mask is > this
       min_mask_area           keep masks of at least this many points (an empty mask is never kept)
-    generate / generate_packed take SAM's min_mask_region_area as a keyword (default 0: off).
-    The model must be in eval mode.  The candidate count points_per_cloud * 3 is limited to 16384."""
+      crop_n_layers           crop layers (0: off; at most 3): layer i splits each axis of the bounding box into 2^i crops
+      crop_nms_thresh         mask-IoU threshold of the NMS across crops
+      crop_overlap_ratio      overlap of neighbouring crops, as a fraction of the bounding box extent per crop count (< 1)
+      crop_n_points_downscale_factor  layer i uses points_per_cloud // factor^i prompts per crop
+    generate / generate_packed take SAM's min_mask_region_area and the four crop_* parameters above as keywords, with
+    SAM's defaults (min_mask_region_area = 0 and crop_n_layers = 0: off).
+    The model must be in eval mode.  The candidate count points_per_cloud * 3 is limited to 16384, and with crop layers
+    the kept masks of all crops together as well (ValueError at the final read)."""
 
     mask_threshold = 0.0  # a point is in the mask when its logit is > 0 (as in predict_masks' callers)
     # neighbours per point of the kNN graph that defines connectivity for min_mask_region_area (the analogue of SAM's
     # 8-connected pixel grid); the graph is undirected, so a point's degree can be higher
     region_neighbors = 8
+    # a crop's candidate is dropped when it holds a point within this fraction of the bounding box extent of an interior
+    # face of the crop (SAM's is_box_near_crop_edge, atol = 20 pixels)
+    crop_edge_margin = 0.02
 
     def __init__(self, model, points_per_cloud: int = 1024, points_per_batch: int = 64, pred_iou_thresh: float = 0.88,
                  stability_score_thresh: float = 0.95, stability_score_offset: float = 1.0, mask_nms_thresh: float = 0.7,
@@ -75,10 +100,105 @@ class PointCloudMaskGenerator:
             raise ValueError(f"{name} must be [N, 3] or [1, N, 3] (one cloud per call), got {tuple(t.shape)}")
         return t.float().contiguous()
 
-    def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
-        """Enqueue the whole generation on the current stream; nothing here waits for the device."""
+    def _generate_one(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None) -> Dict[str, torch.Tensor]:
+        """Generation on one cloud [1, N, 3] (the whole cloud, or one crop's renormalised cloud): encode, P FPS prompts,
+        batched multimask decode, candidates, the crop's edge filter when `edge` is given, mask NMS."""
+        m, dev, N, Bp = self.model, xyz.device, xyz.shape[1], self.points_per_batch
+        enc = m._encode(xyz, rgb)
+        point_index, centers = ops.fps(xyz, P)
+        labels = torch.ones((min(Bp, P), 1), dtype=torch.int64, device=dev)
+        cand, C = None, None
+        for s in range(0, P, Bp):
+            e = min(P, s + Bp)
+            masks, iou = m._decode_unchecked(enc, centers[0, s:e].unsqueeze(1), labels[: e - s], None, True)
+            if cand is None:
+                C = masks.shape[1]
+                K = P * C
+                cand = (torch.empty((K, ops.mask_words(N)), dtype=torch.int32, device=dev),
+                        torch.empty(K, dtype=torch.int32, device=dev), torch.empty(K, dtype=torch.float32, device=dev),
+                        torch.empty(K, dtype=torch.float32, device=dev))
+            ops.mask_candidates(masks, iou, mask_threshold=self.mask_threshold,
+                                stability_offset=self.stability_score_offset, pred_iou_thresh=self.pred_iou_thresh,
+                                stability_thresh=self.stability_score_thresh, min_area=self.min_mask_area, out=cand,
+                                base=s * C)
+        bits, area, stab, score = cand
+        if edge is not None:
+            ops.crop_edge_filter(bits, score, edge)
+        keep, keep_count = ops.mask_nms(bits, area, score, self.mask_nms_thresh)
+        return dict(bits=bits, area=area, stability=stab, score=score, keep=keep, keep_count=keep_count,
+                    point_index=point_index[0], centers=centers[0], slots=C, device=dev)
+
+    @staticmethod
+    def _crop_args(crop_n_layers, crop_nms_thresh, crop_overlap_ratio, crop_n_points_downscale_factor) -> CropArgs:
+        if not 0 <= crop_n_layers <= ops.CROP_MAX_LAYERS:
+            raise ValueError(f"crop_n_layers must be in 0..{ops.CROP_MAX_LAYERS}, got {crop_n_layers}")
+        if not 0 <= crop_overlap_ratio < 1:
+            raise ValueError(f"crop_overlap_ratio must be in [0, 1), got {crop_overlap_ratio}")
+        if crop_n_points_downscale_factor < 1:
+            raise ValueError(f"crop_n_points_downscale_factor must be >= 1, got {crop_n_points_downscale_factor}")
+        if not 0 <= crop_nms_thresh <= 1:
+            raise ValueError(f"crop_nms_thresh must be in [0, 1], got {crop_nms_thresh}")
+        return CropArgs(int(crop_n_layers), float(crop_nms_thresh), float(crop_overlap_ratio), int(crop_n_points_downscale_factor))
+
+    def _crop_prompts(self, factor: int, layer: int, count: int) -> int:
+        return min(max(1, self.points_per_cloud // factor ** layer), count)
+
+    def _enqueue_crops(self, xyz: torch.Tensor, rgb: torch.Tensor, crop: CropArgs, keep_states: bool) -> Dict[str, torch.Tensor]:
+        """Crop layers: the layout, one host read of the crop point counts, generation per crop (layer 0 = the cloud as
+        given), every crop's kept masks lifted to the cloud, then mask NMS across crops (score = layer).  st["crops"] lists
+        the crops that ran (crop, layer, points, prompts); with keep_states, also each crop's generation state (candidates,
+        keep list, FPS prompts) and its global point indices, which otherwise are freed as soon as the crop is lifted."""
+        dev, N = xyz.device, xyz.shape[1]
+        boxes, counts = ops.crop_layout(xyz, crop.n_layers, crop.overlap_ratio)
+        counts_h = counts.tolist()  # the first of the two host synchronisations
+        min_points = self.model._group_shape()[0]
+        runs, first, n = [(0, 0, N)], 1, 8  # (crop, layer, points)
+        for layer in range(1, crop.n_layers + 1):
+            runs += [(t, layer, counts_h[t]) for t in range(first, first + n) if counts_h[t] >= min_points]
+            first, n = first + n, n * 8
+        crops, lifted = [], None
+        offsets = torch.zeros(len(runs) + 1, dtype=torch.int32, device=dev)
+        overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+        for k, (t, layer, count) in enumerate(runs):
+            P = self._crop_prompts(crop.downscale, layer, count)
+            if layer == 0:
+                idx = torch.arange(N, dtype=torch.int32, device=dev)
+                cs = self._generate_one(xyz, rgb, P)
+            else:
+                idx, cx, cr, edge = ops.crop_gather(xyz, rgb, boxes, t, count, self.crop_edge_margin)
+                cs = self._generate_one(cx, cr, P, edge)
+            if lifted is None:
+                C = cs["slots"]
+                cap = min(ops.NMS_MAX_CANDIDATES, C * sum(self._crop_prompts(crop.downscale, l, c) for _, l, c in runs))
+                W = ops.mask_words(N)
+                lifted = (torch.empty((cap, W), dtype=torch.int32, device=dev), torch.empty(cap, dtype=torch.int32, device=dev),
+                          torch.empty(cap, dtype=torch.float32, device=dev), torch.empty(cap, dtype=torch.float32, device=dev),
+                          torch.empty(cap, dtype=torch.int64, device=dev), torch.empty(cap, dtype=torch.int32, device=dev),
+                          torch.empty(cap, dtype=torch.int32, device=dev),
+                          torch.full((cap,), float("-inf"), dtype=torch.float32, device=dev))
+            ops.crop_uncrop((cs["bits"], cs["area"], cs["stability"], cs["score"]), cs["keep"], cs["keep_count"], idx,
+                            cs["point_index"], cs["slots"], t, float(layer), offsets, k, lifted, overflow, N)
+            info = dict(crop=t, layer=layer, points=count, prompts=P)
+            crops.append(dict(cs, idx=idx, **info) if keep_states else info)
+        gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore = lifted
+        if len(runs) > 1:
+            keep, keep_count = ops.mask_nms(gbits, garea, gscore, crop.nms_thresh)
+        else:
+            keep = torch.arange(gbits.shape[0], dtype=torch.int32, device=dev)
+            keep_count = torch.clamp(offsets[1:], max=gbits.shape[0])
+        return dict(bits=gbits, area=garea, score=giou, stability=gstab, keep=keep, keep_count=keep_count, prompt=gprompt,
+                    mask_slot=gslot, crop=gcrop, crop_score=gscore, crop_boxes=boxes, crop_counts=counts, crops=crops,
+                    overflow=overflow, lifted_count=offsets[-1:], xyz=xyz[0], device=dev)
+
+    def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
+                 crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
+                 crop_n_points_downscale_factor: int = 1, keep_crop_states: bool = False) -> Dict[str, torch.Tensor]:
+        """Enqueue the whole generation on the current stream.  Without crop layers nothing here waits for the device; with
+        them, the crop point counts are read once.  keep_crop_states keeps every crop's generation state in st["crops"]
+        (for inspection; it holds each crop's candidate masks until the state is dropped)."""
         if min_mask_region_area < 0:
             raise ValueError(f"min_mask_region_area must be >= 0, got {min_mask_region_area}")
+        crop = self._crop_args(crop_n_layers, crop_nms_thresh, crop_overlap_ratio, crop_n_points_downscale_factor)
         region_area = int(min_mask_region_area)
         m = self.model
         if m.training:
@@ -86,33 +206,15 @@ class PointCloudMaskGenerator:
         xyz, rgb = self._cloud(xyz, "xyz"), self._cloud(rgb, "rgb")
         if xyz.shape[1] != rgb.shape[1]:
             raise ValueError("xyz and rgb must have the same number of points")
-        dev, N = xyz.device, xyz.shape[1]
-        P, Bp = min(self.points_per_cloud, N), self.points_per_batch
+        N = xyz.shape[1]
         with torch.no_grad():
-            enc = m._encode(xyz, rgb)
-            point_index, centers = ops.fps(xyz, P)
-            labels = torch.ones((min(Bp, P), 1), dtype=torch.int64, device=dev)
-            cand, C = None, None
-            for s in range(0, P, Bp):
-                e = min(P, s + Bp)
-                masks, iou = m._decode_unchecked(enc, centers[0, s:e].unsqueeze(1), labels[: e - s], None, True)
-                if cand is None:
-                    C = masks.shape[1]
-                    K = P * C
-                    cand = (torch.empty((K, ops.mask_words(N)), dtype=torch.int32, device=dev),
-                            torch.empty(K, dtype=torch.int32, device=dev), torch.empty(K, dtype=torch.float32, device=dev),
-                            torch.empty(K, dtype=torch.float32, device=dev))
-                ops.mask_candidates(masks, iou, mask_threshold=self.mask_threshold,
-                                    stability_offset=self.stability_score_offset, pred_iou_thresh=self.pred_iou_thresh,
-                                    stability_thresh=self.stability_score_thresh, min_area=self.min_mask_area, out=cand,
-                                    base=s * C)
-            bits, area, stab, score = cand
-            keep, keep_count = ops.mask_nms(bits, area, score, self.mask_nms_thresh)
-            st = dict(bits=bits, area=area, stability=stab, score=score, keep=keep, keep_count=keep_count,
-                      point_index=point_index[0], centers=centers[0], slots=C, device=dev)
+            if crop.n_layers > 0:
+                st = self._enqueue_crops(xyz, rgb, crop, keep_crop_states)
+            else:
+                st = self._generate_one(xyz, rgb, min(self.points_per_cloud, N))
             if region_area > 0:
                 nbr, _ = ops.knn(xyz, xyz, min(self.region_neighbors + 1, N))
-                rbits, rarea, rscore = ops.mask_regions(bits, keep, keep_count, nbr, region_area)
+                rbits, rarea, rscore = ops.mask_regions(st["bits"], st["keep"], st["keep_count"], nbr, region_area)
                 rkeep, rcount = ops.mask_nms(rbits, rarea, rscore, self.mask_nms_thresh)
                 st.update(region_bits=rbits, region_area=rarea, region_score=rscore, region_keep=rkeep, region_count=rcount)
         return st
@@ -123,11 +225,15 @@ class PointCloudMaskGenerator:
         encoder, then select the kept candidates (on the device).  After the small-region stage the count is the second
         NMS's, its keep list holds ranks of the first, and bits / area come from the post-processed masks."""
         flag = engine.bad_flag(st["device"])
-        regions = "region_keep" in st
-        n, bad = (int(v) for v in torch.cat([st["region_count" if regions else "keep_count"], flag]).tolist())
+        regions, crops = "region_keep" in st, "crops" in st
+        reads = [st["region_count" if regions else "keep_count"], flag] + ([st["overflow"]] if crops else [])
+        n, bad, *over = (int(v) for v in torch.cat(reads).tolist())
         if bad:
             flag.zero_()
             raise ValueError("Input coordinates must be normalized to [-1, 1].")
+        if over and over[0]:
+            raise ValueError(f"crop layers: the kept masks of all crops exceed the {st['bits'].shape[0]} lifted slots; "
+                             "lower points_per_cloud or crop_n_layers, or raise crop_n_points_downscale_factor")
         if regions:
             rank = st["region_keep"][:n].long()
             sel = st["keep"][rank].long()
@@ -135,12 +241,19 @@ class PointCloudMaskGenerator:
         else:
             sel = st["keep"][:n].long()
             bits, area = st["bits"][sel], st["area"][sel]
+        if crops:
+            prompt = st["prompt"][sel]
+            return dict(bits=bits, area=area, predicted_iou=st["score"][sel], stability_score=st["stability"][sel],
+                        point_index=prompt, point_coords=st["xyz"][prompt], mask_slot=st["mask_slot"][sel].long(),
+                        crop_box=st["crop_boxes"][st["crop"][sel].long()])
         z = torch.div(sel, st["slots"], rounding_mode="floor")
         return dict(bits=bits, area=area, predicted_iou=st["score"][sel],
                     stability_score=st["stability"][sel], point_index=st["point_index"][z], point_coords=st["centers"][z],
                     mask_slot=sel - z * st["slots"])
 
-    def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
+    def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
+                        crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
+                        crop_n_points_downscale_factor: int = 1) -> Dict[str, torch.Tensor]:
         """Masks of one cloud as device tensors (K = number of kept masks, W = ceil(N / 32)):
         bits [K, W] int32 (point n is bit n % 32 of word n // 32), area [K] int32, predicted_iou [K], stability_score [K],
         point_index [K] int64 (index of the prompt point in the cloud), point_coords [K, 3], mask_slot [K] (0..2: which
@@ -152,15 +265,32 @@ class PointCloudMaskGenerator:
         A points removed (if no island reaches A, the largest stays), and mask NMS runs again on the results with
         unchanged masks ranked before changed ones (ties in the first order).  So the order is: unchanged masks, then
         changed ones, each in score order.  bits and area are the post-processed ones; predicted_iou and
-        stability_score stay the model's."""
-        return self._finish(self._enqueue(xyz, rgb, min_mask_region_area=min_mask_region_area))
+        stability_score stay the model's.
 
-    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> List[Dict]:
+        crop_n_layers > 0: the masks of all crops, in global point indices, merged by mask NMS across crops in which masks
+        of deeper layers rank first (then by crop, then by score within the crop); min_mask_region_area then applies to
+        the merged set.  An extra field crop_box [K, 6] (x0, y0, z0, x1, y1, z1 in the input's coordinates) gives each
+        mask's crop; layer 0's box is the bounding box."""
+        return self._finish(self._enqueue(xyz, rgb, min_mask_region_area=min_mask_region_area, crop_n_layers=crop_n_layers,
+                                          crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
+                                          crop_n_points_downscale_factor=crop_n_points_downscale_factor))
+
+    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
+                 crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
+                 crop_n_points_downscale_factor: int = 1) -> List[Dict]:
         """SAM's record list, in the order of generate_packed: segmentation (bool [N] numpy), area, predicted_iou,
-        stability_score, point_coords ([[x, y, z]]), point_index."""
+        stability_score, point_coords ([[x, y, z]]), point_index, and crop_box ([x0, y0, z0, x1, y1, z1]) with crop
+        layers."""
         N = self._cloud(xyz, "xyz").shape[1]
-        out = {k: v.cpu().numpy() for k, v in self.generate_packed(xyz, rgb, min_mask_region_area=min_mask_region_area).items()}
+        out = self.generate_packed(xyz, rgb, min_mask_region_area=min_mask_region_area, crop_n_layers=crop_n_layers,
+                                   crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
+                                   crop_n_points_downscale_factor=crop_n_points_downscale_factor)
+        out = {k: v.cpu().numpy() for k, v in out.items()}
         seg = np.unpackbits(out["bits"].astype("<i4").view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
-        return [dict(segmentation=seg[i], area=int(out["area"][i]), predicted_iou=float(out["predicted_iou"][i]),
+        recs = [dict(segmentation=seg[i], area=int(out["area"][i]), predicted_iou=float(out["predicted_iou"][i]),
                      stability_score=float(out["stability_score"][i]), point_coords=[out["point_coords"][i].tolist()],
                      point_index=int(out["point_index"][i])) for i in range(len(seg))]
+        if "crop_box" in out:
+            for r, box in zip(recs, out["crop_box"]):
+                r["crop_box"] = box.tolist()
+        return recs

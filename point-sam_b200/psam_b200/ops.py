@@ -401,3 +401,70 @@ def mask_regions(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tenso
                                         nv.ptr(bits_out), nv.ptr(area_out), nv.ptr(score_out), nv.ptr(ws), nv.stream()),
              "mask_regions")
     return bits_out, area_out, score_out
+
+
+# ------------------------------------------------------------------------------------------------
+# crop layers of automatic mask generation
+# ------------------------------------------------------------------------------------------------
+CROP_MAX_LAYERS = 3
+
+
+def crop_total(n_layers: int) -> int:
+    """Crops of layers 0 .. n_layers: sum of 8^i."""
+    return sum(8 ** i for i in range(n_layers + 1))
+
+
+def crop_layout(xyz: torch.Tensor, n_layers: int, overlap_ratio: float):
+    """Crop boxes and point counts of every layer (psam_crop_layout_f32).  xyz [N, 3] or [1, N, 3].  Returns (boxes [T, 6]
+    fp32, counts [T] int32: -1 marks a box equal to an earlier one of its layer); both stay on the device."""
+    x = xyz.reshape(-1, 3).float().contiguous()
+    T = crop_total(n_layers)
+    boxes = torch.empty((T, 6), dtype=torch.float32, device=x.device)
+    counts = torch.empty(T, dtype=torch.int32, device=x.device)
+    nv.check(nv.lib().psam_crop_layout_f32(nv.ptr(x), x.shape[0], int(n_layers), float(overlap_ratio), nv.ptr(boxes), nv.ptr(counts),
+                                           nv.stream()), "crop_layout")
+    return boxes, counts
+
+
+def crop_gather(xyz: torch.Tensor, rgb: torch.Tensor, boxes: torch.Tensor, crop: int, count: int, edge_margin: float):
+    """The crop cloud of crop `crop` with `count` points (its entry of crop_layout's counts), psam_crop_gather_f32.  Returns
+    (idx [count] int32 global indices in ascending order, xyz [1, count, 3] renormalised, rgb [1, count, 3], edge
+    [mask_words(count)] int32: the points near an interior face of the crop)."""
+    x, c = xyz.reshape(-1, 3).float().contiguous(), rgb.reshape(-1, 3).float().contiguous()
+    N, dev = x.shape[0], x.device
+    idx = torch.empty(count, dtype=torch.int32, device=dev)
+    xo = torch.empty((1, count, 3), dtype=torch.float32, device=dev)
+    co = torch.empty((1, count, 3), dtype=torch.float32, device=dev)
+    edge = torch.empty(mask_words(count), dtype=torch.int32, device=dev)
+    ws = torch.empty(nv.lib().psam_crop_gather_workspace_bytes(N), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_crop_gather_f32(nv.ptr(x), nv.ptr(c), N, nv.ptr(boxes), int(crop), boxes.shape[0], float(edge_margin),
+                                           int(count), nv.ptr(idx), nv.ptr(xo), nv.ptr(co), nv.ptr(edge), nv.ptr(ws), nv.stream()),
+             "crop_gather")
+    return idx, xo, co, edge
+
+
+def crop_edge_filter(bits: torch.Tensor, score: torch.Tensor, edge: torch.Tensor):
+    """score[k] = -inf in place for every candidate whose mask bits[k] touches the crop's edge bitset (psam_crop_edge_filter)."""
+    K, W = bits.shape
+    if edge.numel() != W or score.numel() != K:
+        raise ValueError(f"crop_edge_filter: edge has {edge.numel()} words and score {score.numel()} entries for bits {tuple(bits.shape)}")
+    nv.check(nv.lib().psam_crop_edge_filter(nv.ptr(bits) if K else None, K, W, nv.ptr(edge) if K else None,
+                                            nv.ptr(score) if K else None, nv.stream()), "crop_edge_filter")
+
+
+def crop_uncrop(cand, keep: torch.Tensor, keep_count: torch.Tensor, idx: torch.Tensor, prompt_index: torch.Tensor, slots: int,
+                crop: int, layer_score: float, offsets: torch.Tensor, k: int, out, overflow: torch.Tensor, N: int):
+    """Append the kept masks keep[:keep_count] of one crop to the global set (psam_crop_uncrop) of a cloud of N points.
+    cand = (bits [K, W], area, stability, score) of mask_candidates on the crop's idx.numel() points; prompt_index [P] int64
+    (crop-local FPS indices);
+    offsets [>= k + 2] int32 device running offsets: reads offsets[k], writes offsets[k + 1]; out = (gbits [cap, Wg] int32,
+    area, iou, stability, prompt int64, slot, crop int32, score fp32), each of length cap.  Sets overflow[0] = 1 when the
+    set outgrows cap."""
+    bits, area, stab, score = cand
+    gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore = out
+    cap, Wg = gbits.shape
+    nv.check(nv.lib().psam_crop_uncrop(nv.ptr(bits), nv.ptr(area), nv.ptr(score), nv.ptr(stab), keep.shape[0], bits.shape[1], nv.ptr(keep),
+                                       nv.ptr(keep_count), nv.ptr(idx), idx.shape[0], nv.ptr(prompt_index.reshape(-1)), int(slots), int(crop),
+                                       float(layer_score), int(N), Wg, cap, nv.ptr(offsets[k:]), nv.ptr(offsets[k + 1:]), nv.ptr(gbits),
+                                       nv.ptr(garea), nv.ptr(giou), nv.ptr(gstab), nv.ptr(gprompt), nv.ptr(gslot), nv.ptr(gcrop),
+                                       nv.ptr(gscore), nv.ptr(overflow), nv.stream()), "crop_uncrop")

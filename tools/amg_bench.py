@@ -16,7 +16,14 @@ candidate; by default the IoU and stability filters are off (every non-empty mas
 per cloud of generate_packed with the stage, against the same without it measured alternately in the same run, the kernel
 time of each op of the stage (kNN graph, mask_regions, second NMS; torch.profiler over 10 launches of the op alone on the
 generator's own inputs, separate run), and the changed and kept counts.  With the default 0 the output is unchanged.
-usage: python tools/amg_bench.py [--hier] [--steps 10] [--warmup 2] [--sam-thresholds] [--min-region-area 0]"""
+
+--crop-n-layers L (> 0) adds a "crops" object for SAM's crop layers (crop_n_layers = L, crop_n_points_downscale_factor =
+--crop-downscale): ms per cloud with crops against the same generator without them, alternately in the same run, the
+crops that ran with their point and prompt counts, and the kernel time of each new op over all crops of one cloud
+(torch.profiler, each op alone on the generator's own inputs), with their share of the cloud's time.  The kNN graph of
+min_mask_region_area is profiled at this N for reference.  --kind kitti uses the flattened scene-like synthetic cloud.
+usage: python tools/amg_bench.py [--hier] [--steps 10] [--warmup 2] [--sam-thresholds] [--min-region-area 0]
+                                 [--crop-n-layers 0] [--crop-downscale 1] [--kind ball] [--points 32768]"""
 import argparse
 import json
 import os
@@ -45,6 +52,9 @@ ap.add_argument("--prompts", type=int, default=1024)
 ap.add_argument("--batch", type=int, default=64)
 ap.add_argument("--sam-thresholds", action="store_true")
 ap.add_argument("--min-region-area", type=int, default=0)
+ap.add_argument("--crop-n-layers", type=int, default=0)
+ap.add_argument("--crop-downscale", type=int, default=1)
+ap.add_argument("--kind", default="ball", choices=["ball", "kitti"])
 a = ap.parse_args()
 if not torch.cuda.is_available():
     sys.exit("amg_bench: needs a CUDA device")
@@ -64,7 +74,7 @@ torch.manual_seed(1234)
 model = (build_point_sam_hier() if a.hier else build_point_sam("eva02_large_patch14_448", 512, 64)).to(dev).eval()
 kw = {} if a.sam_thresholds else dict(pred_iou_thresh=0.0, stability_score_thresh=0.0)
 gen = PointCloudMaskGenerator(model, points_per_cloud=a.prompts, points_per_batch=a.batch, **kw)
-xyz, rgb = (t.to(dev) for t in synth.make_batch(1, a.points, 5, "ball"))
+xyz, rgb = (t.to(dev) for t in synth.make_batch(1, a.points, 5, a.kind))
 N, P, Bp = a.points, a.prompts, a.batch
 rules = dict(mask_threshold=gen.mask_threshold, stability_offset=gen.stability_score_offset, pred_iou_thresh=gen.pred_iou_thresh,
              stability_thresh=gen.stability_score_thresh, min_area=gen.min_mask_area)
@@ -255,6 +265,84 @@ def regions_report(A):
     }
 
 
+def profile_ms(fn, tags, reps=10):
+    """ms per call of fn's kernels whose names contain one of tags (torch.profiler, fn alone)."""
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+    per = {}
+    for evt in prof.events():
+        if evt.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        for tag in tags:
+            if tag in evt.name:
+                per[tag] = per.get(tag, 0.0) + (getattr(evt, "device_time", None) or evt.cuda_time) / 1e3 / reps
+    return {"ms": sum(per.values()), "kernels": per}
+
+
+# ---- crop layers: with / without alternately, the crops, then the new kernels each profiled alone ---------------------
+def crops_report(layers, factor):
+    ck = dict(crop_n_layers=layers, crop_n_points_downscale_factor=factor)
+    ratio, crop_nms, margin = 512 / 1500, 0.7, gen.crop_edge_margin  # SAM's defaults
+    for _ in range(a.warmup):
+        gen.generate_packed(xyz, rgb, **ck)
+    torch.cuda.synchronize()
+    on, off = [], []
+    for _ in range(a.steps):
+        for c, dst in ((ck, on), ({}, off)):
+            t0 = time.perf_counter()
+            gen.generate_packed(xyz, rgb, **c)
+            dst.append((time.perf_counter() - t0) * 1e3)
+    st = gen._enqueue(xyz, rgb, **ck, keep_crop_states=True)
+    out = gen._finish(st)
+    counts = st["crop_counts"].tolist()
+    crops = st["crops"]
+    sub = [c for c in crops if c["layer"] > 0]
+    boxes = st["crop_boxes"]
+    gathered = [ops.crop_gather(xyz, rgb, boxes, c["crop"], counts[c["crop"]], margin) for c in sub]
+    lifted = tuple(st[k] for k in ("bits", "area", "score", "stability", "prompt", "mask_slot", "crop", "crop_score"))
+    offsets = torch.zeros(len(crops) + 1, dtype=torch.int32, device=dev)
+    over = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def uncrop_all():
+        for k, c in enumerate(crops):
+            ops.crop_uncrop((c["bits"], c["area"], c["stability"], c["score"]), c["keep"], c["keep_count"], c["idx"], c["point_index"],
+                            c["slots"], c["crop"], float(c["layer"]), offsets, k, lifted, over, N)
+
+    def edge_all():
+        for c, g in zip(sub, gathered):
+            ops.crop_edge_filter(c["bits"], c["score"].clone(), g[3])
+
+    k1 = min(gen.region_neighbors + 1, N)
+    kernels = {
+        "crop_layout": profile_ms(lambda: ops.crop_layout(xyz, layers, ratio), ("crop_layout_kernel", "crop_count_kernel")),
+        "crop_gather (all crops)": profile_ms(lambda: [ops.crop_gather(xyz, rgb, boxes, c["crop"], counts[c["crop"]], margin)
+                                                       for c in sub], ("crop_gather",)),
+        "crop_edge_filter (all crops)": profile_ms(edge_all, ("crop_edge_filter_kernel",)),
+        "crop_uncrop (all crops)": profile_ms(uncrop_all, ("crop_uncrop_kernel",)),
+        "nms_across_crops": profile_ms(lambda: ops.mask_nms(st["bits"], st["area"], st["crop_score"], crop_nms),
+                                       ("nms_order_kernel", "nms_pairs_kernel", "nms_scan_kernel")),
+        "knn_graph (min_mask_region_area, not run here)": profile_ms(lambda: ops.knn(xyz, xyz, k1), ("knn_kernel",), reps=3),
+    }
+    new_ms = sum(v["ms"] for k, v in kernels.items() if not k.startswith("knn_graph"))
+    med_on = float(np.median(on))
+    return {
+        "crop_n_layers": layers, "crop_n_points_downscale_factor": factor,
+        "ms_per_cloud_with": med_on, "ms_per_cloud_without": float(np.median(off)),
+        "ms_per_cloud_with_range": [min(on), max(on)], "ms_per_cloud_without_range": [min(off), max(off)],
+        "crops_run": len(crops), "points_per_crop": [c["points"] for c in crops], "prompts_per_crop": [c["prompts"] for c in crops],
+        "crops_skipped": sum(1 for t in range(1, len(counts)) if t not in {c["crop"] for c in crops}),
+        "lifted_masks": int(st["lifted_count"].item()), "kept_masks": int(out["area"].shape[0]),
+        "kept_from_deeper_layers": int((out["crop_box"] != st["crop_boxes"][0]).any(1).sum().item()),
+        "kernel_ms": kernels, "new_kernels_ms": new_ms, "new_kernels_share": new_ms / med_on,
+    }
+
+
 if a.min_region_area > 0:
     line["regions"] = regions_report(a.min_region_area)
+if a.crop_n_layers > 0:
+    line["crops"] = crops_report(a.crop_n_layers, a.crop_downscale)
 print(json.dumps(line))
