@@ -320,6 +320,16 @@ int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z,
                              float stability_offset, float pred_iou_thresh, float stability_thresh, int min_area,
                              long long base, int W, uint32_t* bits, int* area, float* stability, float* score,
                              cudaStream_t stream);
+/* The same for B clouds in one launch: logits [B * Zc, C, N] and iou_preds [B * Zc, C], where rows b * Zc .. b * Zc + Zc - 1
+ * belong to cloud b (the mask decoder's layout for B encoded clouds).  Row z = b * Zc + j, output c goes to slot
+ *   b * cloud_stride + base + j * C + c,
+ * with the same rules and the same fp32 arithmetic, so every cloud's slots equal psam_mask_candidates_f32 on its own rows.
+ * psam_mask_candidates_f32 is the case B = 1, Zc = Z.  B >= 1, Zc >= 1, B * Zc * C < 2^31, and for B > 1
+ * cloud_stride >= base + Zc * C (the clouds' blocks do not overlap).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_candidates_batched_f32(const float* logits, const float* iou_preds, int B, int Zc, int C, int N,
+                                     float mask_threshold, float stability_offset, float pred_iou_thresh, float stability_thresh,
+                                     int min_area, long long base, long long cloud_stride, int W, uint32_t* bits, int* area,
+                                     float* stability, float* score, cudaStream_t stream);
 
 /* Greedy mask-IoU non-maximum suppression over K <= 16384 candidate slots of W words each (the output of
  * psam_mask_candidates_f32).  Stands in for the duplicate-removal stage of SamAutomaticMaskGenerator._process_batch /
@@ -334,6 +344,17 @@ int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z,
 size_t psam_mask_nms_workspace_bytes(int K, int W);
 int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh, int* keep,
                   int* keep_count, void* workspace, cudaStream_t stream);
+/* psam_mask_nms on B clouds of K candidate slots each, in the same three launches: bits [B, K, W], area / score [B, K];
+ * keep [B, K] holds each cloud's kept slot indices (within the cloud, 0 .. K-1) in score order, keep_count [B] their counts.
+ * Each cloud's result equals psam_mask_nms on its own slice: the order, the tie-break and the IoU arithmetic are the same.
+ * The order and scan kernels run one CTA per cloud; the pairwise tiles past a cloud's own valid count exit at once.
+ * workspace: psam_mask_nms_batched_workspace_bytes(B, K, W) = B * psam_mask_nms_workspace_bytes(K, W) bytes, 16-byte aligned:
+ * per cloud a K x ceil(K/64) matrix of 64-bit suppression words plus the order (1.2 MB at K = 3072, about 34 MB at
+ * K = 16383).  psam_mask_nms is the case B = 1.  1 <= B <= 65535 (0 bytes outside), 0 <= K <= 16384.
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_mask_nms_batched_workspace_bytes(int B, int K, int W);
+int psam_mask_nms_batched(const uint32_t* bits, const int* area, const float* score, int B, int K, int W, float nms_thresh,
+                          int* keep, int* keep_count, void* workspace, cudaStream_t stream);
 
 /* Small-region post-processing of the kept masks: segment-anything's SamAutomaticMaskGenerator.postprocess_small_regions /
  * remove_small_regions (min_mask_region_area), restated for a point cloud of N points.
@@ -360,6 +381,18 @@ size_t psam_mask_regions_workspace_bytes(int K, int N);
 int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep, const int* keep_count, const long long* nbr,
                       int k1, int min_area, uint32_t* bits_out, int* area_out, float* score_out, void* workspace,
                       cudaStream_t stream);
+/* psam_mask_regions on B clouds of N points in one launch of persistent CTAs over the B * K (cloud, rank) items.  Cloud b's
+ * candidate masks start at bits + b * cloud_slots * W (its keep entries index them), its kNN graph is nbr[b] of nbr
+ * [B, N, k1], its keep list keep[b] of keep [B, K] and its count keep_count[b]; its outputs are row b of bits_out [B, K, W],
+ * area_out [B, K] and score_out [B, K] (score -inf past the cloud's count).  Each cloud's result equals psam_mask_regions
+ * on its own slice.  The label slices of the workspace form are shared by all items of the launch, so the workspace does not
+ * grow with B beyond its cap: psam_mask_regions_batched_workspace_bytes(B, K, N) is psam_mask_regions_workspace_bytes' formula
+ * with min(B * K, 132, 24 MiB / 4N) slices.  psam_mask_regions is the case B = 1 (cloud_slots unused).  B >= 1,
+ * cloud_slots >= 1 when B > 1.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_mask_regions_batched_workspace_bytes(int B, int K, int N);
+int psam_mask_regions_batched(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* keep,
+                              const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out,
+                              int* area_out, float* score_out, void* workspace, cudaStream_t stream);
 
 /* ---- crop layers of automatic mask generation (SAM's crop_n_layers) ------------------------------ */
 /* Layout.  Layer 0 is the whole cloud.  Layer i >= 1 splits every axis a of the cloud's axis-aligned bounding box

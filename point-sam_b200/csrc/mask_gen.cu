@@ -1,16 +1,18 @@
 // Automatic mask generation ("segment everything"): candidate extraction from multimask decoder logits and greedy
-// mask-IoU NMS, all on the device.  The semantics are stated in include/psam_b200.h.
+// mask-IoU NMS, all on the device.  The semantics are stated in include/psam_b200.h.  Every kernel takes a cloud
+// dimension: the single-cloud entry points are the B = 1 case of the batched ones.
 //
 //   mask_candidates_kernel   one CTA per logit row: a single streaming pass (128-bit loads where aligned) produces the
 //                            bit-packed mask, the three threshold counts, the stability score and the filtered score.
-//   nms_order_kernel         one CTA: bitonic sort of the (score desc, slot asc) keys in shared memory, valid count.
-//   nms_pairs_kernel         64 x 64 tiles of sorted positions (upper triangle): AND + popc over the bit-packed masks
-//                            staged through shared memory, comparisons turned into 64-bit suppression words by ballots.
-//   nms_scan_kernel          one CTA: greedy walk in blocks of 64; one warp resolves a block against its diagonal
+//   nms_order_kernel         one CTA per cloud: bitonic sort of the (score desc, slot asc) keys in shared memory, valid count.
+//   nms_pairs_kernel         64 x 64 tiles of sorted positions (upper triangle) per cloud (grid.z): AND + popc over the
+//                            bit-packed masks staged through shared memory, comparisons turned into 64-bit suppression
+//                            words by ballots.
+//   nms_scan_kernel          one CTA per cloud: greedy walk in blocks of 64; one warp resolves a block against its diagonal
 //                            words, then every thread ORs the kept rows into the "removed" bitset.
-//   mask_regions_kernel<S>   one CTA per kept mask: lock-free union-find over the kNN graph, first on the points outside
-//                            the mask (small holes are filled), then on the mask (small islands are removed); labels in
-//                            shared memory (S = true, N <= 49152) or in a per-CTA slice of the workspace.
+//   mask_regions_kernel<S>   one CTA per (cloud, kept mask): lock-free union-find over the kNN graph, first on the points
+//                            outside the mask (small holes are filled), then on the mask (small islands are removed); labels
+//                            in shared memory (S = true, N <= 49152) or in a per-CTA slice of the workspace.
 #include <math.h>
 #include "psam_common.cuh"
 #include "../../include/psam_b200.h"
@@ -22,6 +24,7 @@ constexpr int kNmsMaxK = 16384;
 constexpr int kTile = 64;       // sorted positions per tile side / per scan block
 constexpr int kTileWords = 32;  // mask words staged per shared-memory round
 constexpr int kScanThreads = 512;
+constexpr int kNmsMaxClouds = 65535;  // grid.z of nms_pairs_kernel
 
 __device__ __forceinline__ bool candidate_survives(float iou, float stab, int area, float iou_t, float stab_t, int min_area) {
     if (!(iou == iou)) return false;  // a NaN predicted IoU is never kept
@@ -34,14 +37,16 @@ template <bool VEC>
 __global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const float* __restrict__ logits,
                                                                        const float* __restrict__ iou_preds, int N,
                                                                        float thr, float thr_hi, float thr_lo, float iou_t,
-                                                                       float stab_t, int min_area, long long base, int W,
+                                                                       float stab_t, int min_area, long long base,
+                                                                       int rows_per_cloud, long long cloud_stride, int W,
                                                                        uint32_t* __restrict__ bits, int* __restrict__ area_out,
                                                                        float* __restrict__ stab_out, float* __restrict__ score_out) {
     psam::pdl_prologue();
     constexpr int U = 4;  // warp iterations whose loads are issued together
     const int row = blockIdx.x;
     const float* rp = logits + (size_t)row * N;
-    const long long slot = base + row;
+    const int cloud = row / rows_per_cloud;  // rows of cloud b are b * rows_per_cloud .. (b + 1) * rows_per_cloud
+    const long long slot = cloud * cloud_stride + base + (row - cloud * rows_per_cloud);
     uint32_t* bp = bits + (size_t)slot * W;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     int n_area = 0, n_hi = 0, n_lo = 0;
@@ -129,10 +134,31 @@ __global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const flo
     }
 }
 
+// ---- NMS workspace: one block per cloud of cloud_bytes = psam_mask_nms_workspace_bytes(K, W) bytes ---------------
+//   [0, 16)                 the valid count
+//   [16, 16 + order bytes)  the sorted slot order
+//   then                    the K x ceil(K / 64) suppression words
+__host__ __device__ __forceinline__ size_t nms_order_bytes(int K) { return ((size_t)K * sizeof(int) + 15) / 16 * 16; }
+
+struct NmsCloud {
+    int* count;
+    int* order;
+    unsigned long long* mat;
+};
+
+__device__ __forceinline__ NmsCloud nms_cloud(char* ws, size_t cloud_bytes, int K, int b) {
+    char* c = ws + (size_t)b * cloud_bytes;
+    return {reinterpret_cast<int*>(c), reinterpret_cast<int*>(c + 16), reinterpret_cast<unsigned long long*>(c + 16 + nms_order_bytes(K))};
+}
+
 // ---- NMS a: order ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) nms_order_kernel(const float* __restrict__ score, int K, int P2, int* __restrict__ order,
-                                                         int* __restrict__ count) {
+// One CTA per cloud (blockIdx.x); the cloud's K scores start at score + b * K.
+__global__ void __launch_bounds__(1024) nms_order_kernel(const float* __restrict__ score, int K, int P2, char* __restrict__ ws,
+                                                         size_t cloud_bytes) {
     psam::pdl_prologue();
+    const NmsCloud cw = nms_cloud(ws, cloud_bytes, K, blockIdx.x);
+    score += (size_t)blockIdx.x * K;
+    int* __restrict__ order = cw.order;
     extern __shared__ unsigned long long keys[];
     __shared__ int n_valid;
     if (threadIdx.x == 0) n_valid = 0;
@@ -169,20 +195,24 @@ __global__ void __launch_bounds__(1024) nms_order_kernel(const float* __restrict
     }
     __syncthreads();
     for (int i = threadIdx.x; i < K; i += blockDim.x) order[i] = (int)(uint32_t)(keys[i] & 0xffffffffull);
-    if (threadIdx.x == 0) *count = n_valid;
+    if (threadIdx.x == 0) *cw.count = n_valid;
 }
 
 // ---- NMS b: pairwise suppression bits ---------------------------------------------------------------------------
-// Tile (bi, bj), bj >= bi, of sorted positions.  Thread (ty, tx) of 16 x 16 owns rows ty*4 + r and columns tx + 16 c.
-__global__ void __launch_bounds__(256) nms_pairs_kernel(const uint32_t* __restrict__ bits, const int* __restrict__ area, int W,
-                                                        float nms_thresh, const int* __restrict__ order,
-                                                        const int* __restrict__ count_p, unsigned long long* __restrict__ mat,
-                                                        int ldm) {
+// Tile (bi, bj), bj >= bi, of sorted positions of cloud blockIdx.z, whose candidates start at bits + b * K * W and
+// area + b * K.  Thread (ty, tx) of 16 x 16 owns rows ty*4 + r and columns tx + 16 c.
+__global__ void __launch_bounds__(256) nms_pairs_kernel(const uint32_t* __restrict__ bits, const int* __restrict__ area, int K, int W,
+                                                        float nms_thresh, char* __restrict__ ws, size_t cloud_bytes, int ldm) {
     psam::pdl_prologue();
     const int bi = blockIdx.y, bj = blockIdx.x;
     if (bj < bi) return;
-    const int count = *count_p;
-    if (bj * kTile >= count) return;  // beyond the valid candidates (bi <= bj)
+    const NmsCloud cw = nms_cloud(ws, cloud_bytes, K, blockIdx.z);
+    const int count = *cw.count;
+    if (bj * kTile >= count) return;  // beyond the cloud's valid candidates (bi <= bj)
+    const int* __restrict__ order = cw.order;
+    unsigned long long* __restrict__ mat = cw.mat;
+    bits += (size_t)blockIdx.z * K * W;
+    area += (size_t)blockIdx.z * K;
     __shared__ __align__(16) uint32_t sa[kTileWords][kTile];
     __shared__ __align__(16) uint32_t sb[kTileWords][kTile];
     __shared__ int slot_a[kTile], slot_b[kTile], area_a[kTile], area_b[kTile];
@@ -254,14 +284,19 @@ __global__ void __launch_bounds__(256) nms_pairs_kernel(const uint32_t* __restri
 }
 
 // ---- NMS c: greedy scan ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const unsigned long long* __restrict__ mat, int ldm,
-                                                                const int* __restrict__ order, const int* __restrict__ count_p,
+// One CTA per cloud (blockIdx.x): keep + b * K, keep_count + b.
+__global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const char* __restrict__ ws, size_t cloud_bytes, int K, int ldm,
                                                                 int* __restrict__ keep, int* __restrict__ keep_count) {
     psam::pdl_prologue();
     __shared__ unsigned long long removed[kNmsMaxK / kTile];
     __shared__ int kept_rows[kTile];
     __shared__ int n_block, n_kept;
-    const int count = *count_p;
+    const NmsCloud cw = nms_cloud(const_cast<char*>(ws), cloud_bytes, K, blockIdx.x);
+    const unsigned long long* __restrict__ mat = cw.mat;
+    const int* __restrict__ order = cw.order;
+    keep += (size_t)blockIdx.x * K;
+    keep_count += blockIdx.x;
+    const int count = *cw.count;
     const int nb = (count + kTile - 1) / kTile;
     const int tid = threadIdx.x;
     for (int c = tid; c < nb; c += blockDim.x) removed[c] = 0ull;
@@ -311,8 +346,6 @@ __global__ void __launch_bounds__(kScanThreads) nms_scan_kernel(const unsigned l
     if (tid == 0) *keep_count = n_kept;
 }
 
-size_t nms_order_bytes(int K) { return ((size_t)K * sizeof(int) + 15) / 16 * 16; }
-
 // ---- small-region post-processing: connected components over the kNN graph ------------------------------------------
 // One CTA per kept mask (persistent over the ranks).  par[] is a union-find forest over the points of the working set with
 // par[i] <= i at all times, so every root is the smallest point of its component and the forest's final shape does not
@@ -323,11 +356,12 @@ constexpr int kRegionMaxN = 1 << 20;           // the mask words (N / 8 bytes) a
 constexpr long long kRegionL2Bytes = 24ll << 20;  // workspace form: label slices meant to stay L2-resident
 constexpr int kRegionMaxSlices = 132;
 
-// label slices of the workspace form (one per CTA): as many as fit kRegionL2Bytes, at most kRegionMaxSlices and K
-int region_slices(int K, int N) {
+// label slices of the workspace form (one per CTA), shared by all clouds of a launch: as many as fit kRegionL2Bytes, at
+// most kRegionMaxSlices and the number of items
+int region_slices(long long items, int N) {
     long long fit = kRegionL2Bytes / ((long long)N * 4);
     fit = fit < 1 ? 1 : (fit > kRegionMaxSlices ? kRegionMaxSlices : fit);
-    return K < fit ? K : (int)fit;
+    return (int)(items < fit ? items : fit);
 }
 
 __device__ __forceinline__ bool region_member(const uint32_t* sw, int i, int N, bool invert) {
@@ -400,9 +434,12 @@ __device__ void region_components(const uint32_t* sw, bool invert, int N, const 
 
 __device__ __forceinline__ int region_root(const int* par, int i) { return par[i] < 0 ? i : par[i]; }
 
+// Items it = b * K + p of B clouds: cloud b's candidates start at bits + b * cloud_slots * W, its graph at nbr + b * N * k1,
+// its keep list and outputs at b * K; its count is keep_count[b].
 template <bool SMEM>
-__global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint32_t* __restrict__ bits, int K, int W, int N,
-                                                                      const int* __restrict__ keep, const int* __restrict__ keep_count,
+__global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint32_t* __restrict__ bits, long long cloud_slots, int B,
+                                                                      int K, int W, int N, const int* __restrict__ keep,
+                                                                      const int* __restrict__ keep_count,
                                                                       const long long* __restrict__ nbr, int k1, int min_area,
                                                                       uint32_t* __restrict__ bits_out, int* __restrict__ area_out,
                                                                       float* __restrict__ score_out, int* __restrict__ workspace) {
@@ -413,14 +450,16 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
     int* par = SMEM ? reinterpret_cast<int*>(region_smem + ((Wn + 3) & ~3)) : workspace + (size_t)blockIdx.x * N;
     __shared__ int changed, any_small, area_red;
     __shared__ unsigned long long best;  // (size << 32) | ~root: the largest component, smallest root on equal sizes
-    const int count = *keep_count;
     const int lane = threadIdx.x & 31;
-    for (int p = blockIdx.x; p < K; p += gridDim.x) {
-        if (p >= count) {
-            if (threadIdx.x == 0) score_out[p] = -INFINITY;
+    const long long items = (long long)B * K;
+    for (long long it = blockIdx.x; it < items; it += gridDim.x) {
+        const int b = (int)(it / K), p = (int)(it - (long long)b * K);
+        if (p >= keep_count[b]) {
+            if (threadIdx.x == 0) score_out[it] = -INFINITY;
             continue;
         }
-        const uint32_t* src = bits + (size_t)keep[p] * W;
+        const uint32_t* src = bits + ((size_t)b * cloud_slots + keep[it]) * W;
+        const long long* cnbr = nbr + (size_t)b * N * k1;
         for (int w = threadIdx.x; w < Wn; w += blockDim.x) {
             const int tail = N - 32 * w;
             sw[w] = tail >= 32 ? src[w] : src[w] & ((1u << tail) - 1u);
@@ -433,7 +472,7 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
         }
         __syncthreads();
         // 1. holes: components of the complement smaller than min_area join the mask
-        region_components(sw, true, N, nbr, k1, par);
+        region_components(sw, true, N, cnbr, k1, par);
         for (int i = threadIdx.x; i < Wn * 32; i += blockDim.x) {  // a warp owns whole words
             const uint32_t word = sw[i >> 5];
             const bool in = (word >> (i & 31)) & 1u;
@@ -446,7 +485,7 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
         }
         __syncthreads();
         // 2. islands: components of the mask smaller than min_area leave it; if none reaches min_area, the largest stays
-        region_components(sw, false, N, nbr, k1, par);
+        region_components(sw, false, N, cnbr, k1, par);
         for (int i = threadIdx.x; i < N; i += blockDim.x) {
             if (par[i] < 0 && region_member(sw, i, N, false)) {
                 const int size = -par[i];
@@ -467,16 +506,16 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
                 in = none_big ? r == keep_root : -par[r] >= min_area;
             }
             const uint32_t out = __ballot_sync(0xffffffffu, in);
-            if (lane == 0) bits_out[(size_t)p * W + (i >> 5)] = out;
+            if (lane == 0) bits_out[(size_t)it * W + (i >> 5)] = out;
             a += in;
         }
-        for (int w = Wn + threadIdx.x; w < W; w += blockDim.x) bits_out[(size_t)p * W + w] = 0u;
+        for (int w = Wn + threadIdx.x; w < W; w += blockDim.x) bits_out[(size_t)it * W + w] = 0u;
         a = __reduce_add_sync(0xffffffffu, a);
         if (lane == 0 && a) atomicAdd(&area_red, a);
         __syncthreads();
         if (threadIdx.x == 0) {
-            area_out[p] = area_red;
-            score_out[p] = (changed || drop) ? 0.f : 1.f;
+            area_out[it] = area_red;
+            score_out[it] = (changed || drop) ? 0.f : 1.f;
         }
         __syncthreads();  // sw, par and the shared flags are reused by the next rank
     }
@@ -484,21 +523,31 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
 
 }  // namespace
 
+extern "C" int psam_mask_candidates_batched_f32(const float* logits, const float* iou_preds, int B, int Zc, int C, int N,
+                                                float mask_threshold, float stability_offset, float pred_iou_thresh,
+                                                float stability_thresh, int min_area, long long base, long long cloud_stride,
+                                                int W, uint32_t* bits, int* area, float* stability, float* score,
+                                                cudaStream_t stream) {
+    if (!logits || !iou_preds || !bits || !area || !stability || !score) return PSAM_ERR_ARG;
+    if (B <= 0 || Zc <= 0 || C <= 0 || N <= 0 || base < 0 || W < psam::ceil_div(N, 32)) return PSAM_ERR_ARG;
+    if ((long long)B * Zc * C > 0x7fffffffLL) return PSAM_ERR_ARG;
+    if (B > 1 && cloud_stride < base + (long long)Zc * C) return PSAM_ERR_ARG;  // the clouds' slot blocks must not overlap
+    const float thr_hi = mask_threshold + stability_offset, thr_lo = mask_threshold - stability_offset;
+    const bool vec = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(logits) % 16 == 0);
+    auto kernel = vec ? mask_candidates_kernel<true> : mask_candidates_kernel<false>;
+    PSAM_CUDA_TRY(psam::launch(kernel, dim3(B * Zc * C), dim3(kCandThreads), (size_t)0, stream, logits, iou_preds, N, mask_threshold,
+                               thr_hi, thr_lo, pred_iou_thresh, stability_thresh, min_area, base, Zc * C, cloud_stride, W, bits,
+                               area, stability, score));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
 extern "C" int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z, int C, int N, float mask_threshold,
                                         float stability_offset, float pred_iou_thresh, float stability_thresh, int min_area,
                                         long long base, int W, uint32_t* bits, int* area, float* stability, float* score,
                                         cudaStream_t stream) {
-    if (!logits || !iou_preds || !bits || !area || !stability || !score) return PSAM_ERR_ARG;
-    if (Z <= 0 || C <= 0 || N <= 0 || base < 0 || W < psam::ceil_div(N, 32)) return PSAM_ERR_ARG;
-    if ((long long)Z * C > 0x7fffffffLL) return PSAM_ERR_ARG;
-    const float thr_hi = mask_threshold + stability_offset, thr_lo = mask_threshold - stability_offset;
-    const bool vec = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(logits) % 16 == 0);
-    auto kernel = vec ? mask_candidates_kernel<true> : mask_candidates_kernel<false>;
-    PSAM_CUDA_TRY(psam::launch(kernel, dim3(Z * C), dim3(kCandThreads), (size_t)0, stream, logits, iou_preds, N, mask_threshold,
-                               thr_hi, thr_lo, pred_iou_thresh, stability_thresh, min_area, base, W, bits, area, stability,
-                               score));
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
+    return psam_mask_candidates_batched_f32(logits, iou_preds, 1, Z, C, N, mask_threshold, stability_offset, pred_iou_thresh,
+                                            stability_thresh, min_area, base, 0, W, bits, area, stability, score, stream);
 }
 
 extern "C" size_t psam_mask_nms_workspace_bytes(int K, int W) {
@@ -508,66 +557,87 @@ extern "C" size_t psam_mask_nms_workspace_bytes(int K, int W) {
     return 16 + nms_order_bytes(K) + (size_t)K * ldm * sizeof(unsigned long long);
 }
 
-extern "C" int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh,
-                             int* keep, int* keep_count, void* workspace, cudaStream_t stream) {
-    if (!keep || !keep_count || !workspace || K < 0 || K > kNmsMaxK) return PSAM_ERR_ARG;
+extern "C" size_t psam_mask_nms_batched_workspace_bytes(int B, int K, int W) {
+    if (B < 1 || B > kNmsMaxClouds) return 0;
+    return (size_t)B * psam_mask_nms_workspace_bytes(K, W);
+}
+
+extern "C" int psam_mask_nms_batched(const uint32_t* bits, const int* area, const float* score, int B, int K, int W,
+                                     float nms_thresh, int* keep, int* keep_count, void* workspace, cudaStream_t stream) {
+    if (!keep || !keep_count || !workspace || B < 1 || B > kNmsMaxClouds || K < 0 || K > kNmsMaxK) return PSAM_ERR_ARG;
     if (K > 0 && (!bits || !area || !score || W <= 0)) return PSAM_ERR_ARG;
     if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
     char* ws = static_cast<char*>(workspace);
-    int* count = reinterpret_cast<int*>(ws);
-    int* order = reinterpret_cast<int*>(ws + 16);
-    auto* mat = reinterpret_cast<unsigned long long*>(ws + 16 + nms_order_bytes(K));
+    const size_t cloud_bytes = psam_mask_nms_workspace_bytes(K, W);
     const int ldm = (K + kTile - 1) / kTile;
     int P2 = 2;
     while (P2 < K) P2 <<= 1;
     const size_t smem = (size_t)P2 * sizeof(unsigned long long);
     if (smem > 48 * 1024)
         PSAM_CUDA_TRY(cudaFuncSetAttribute(nms_order_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PSAM_CUDA_TRY(psam::launch(nms_order_kernel, dim3(1), dim3(1024), smem, stream, score, K, P2, order, count));
+    PSAM_CUDA_TRY(psam::launch(nms_order_kernel, dim3(B), dim3(1024), smem, stream, score, K, P2, ws, cloud_bytes));
     PSAM_LAUNCH_CHECK();
     if (K > 0) {
-        PSAM_CUDA_TRY(psam::launch(nms_pairs_kernel, dim3(ldm, ldm), dim3(256), (size_t)0, stream, bits, area, W, nms_thresh,
-                                   (const int*)order, (const int*)count, mat, ldm));
+        PSAM_CUDA_TRY(psam::launch(nms_pairs_kernel, dim3(ldm, ldm, B), dim3(256), (size_t)0, stream, bits, area, K, W, nms_thresh, ws,
+                                   cloud_bytes, ldm));
         PSAM_LAUNCH_CHECK();
     }
-    PSAM_CUDA_TRY(psam::launch(nms_scan_kernel, dim3(1), dim3(kScanThreads), (size_t)0, stream, (const unsigned long long*)mat,
-                               ldm, (const int*)order, (const int*)count, keep, keep_count));
+    PSAM_CUDA_TRY(psam::launch(nms_scan_kernel, dim3(B), dim3(kScanThreads), (size_t)0, stream, (const char*)ws, cloud_bytes, K, ldm,
+                               keep, keep_count));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }
 
-extern "C" size_t psam_mask_regions_workspace_bytes(int K, int N) {
-    if (K < 0 || K > kNmsMaxK || N <= 0 || N > kRegionMaxN) return 0;
+extern "C" int psam_mask_nms(const uint32_t* bits, const int* area, const float* score, int K, int W, float nms_thresh,
+                             int* keep, int* keep_count, void* workspace, cudaStream_t stream) {
+    return psam_mask_nms_batched(bits, area, score, 1, K, W, nms_thresh, keep, keep_count, workspace, stream);
+}
+
+extern "C" size_t psam_mask_regions_batched_workspace_bytes(int B, int K, int N) {
+    if (B < 1 || K < 0 || K > kNmsMaxK || N <= 0 || N > kRegionMaxN) return 0;
     if (N <= kRegionSmemMaxN) return 16;
-    const size_t bytes = ((size_t)region_slices(K, N) * N * sizeof(int) + 15) / 16 * 16;
+    const size_t bytes = ((size_t)region_slices((long long)B * K, N) * N * sizeof(int) + 15) / 16 * 16;
     return bytes < 16 ? 16 : bytes;
+}
+
+extern "C" size_t psam_mask_regions_workspace_bytes(int K, int N) { return psam_mask_regions_batched_workspace_bytes(1, K, N); }
+
+extern "C" int psam_mask_regions_batched(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* keep,
+                                         const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out,
+                                         int* area_out, float* score_out, void* workspace, cudaStream_t stream) {
+    if (!keep_count || !nbr || !workspace) return PSAM_ERR_ARG;
+    if (K > 0 && (!bits || !keep || !bits_out || !area_out || !score_out)) return PSAM_ERR_ARG;
+    if (N <= 0 || N > kRegionMaxN || W < psam::ceil_div(N, 32) || k1 < 1 || k1 > N || K < 0 || K > kNmsMaxK || min_area < 1)
+        return PSAM_ERR_ARG;
+    if (B < 1 || cloud_slots < 0 || (B > 1 && cloud_slots < 1)) return PSAM_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
+    if (K == 0) return PSAM_OK;
+    // persistent grid over the B * K items: two CTAs per SM in the shared-memory form, one per label slice (at most one per
+    // SM) otherwise
+    const long long items = (long long)B * K;
+    int dev = 0, sms = 0;
+    PSAM_CUDA_TRY(cudaGetDevice(&dev));
+    PSAM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int grid = N <= kRegionSmemMaxN ? (int)(items < 2 * sms ? items : 2 * sms) : min(region_slices(items, N), sms);
+    const size_t words = (size_t)(psam::ceil_div(N, 32) + 3) / 4 * 4 * sizeof(uint32_t);
+    if (N <= kRegionSmemMaxN) {
+        const size_t smem = words + (size_t)N * sizeof(int);
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<true>, dim3(grid), dim3(kRegionThreads), smem, stream, bits, cloud_slots, B, K,
+                                   W, N, keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out, (int*)nullptr));
+    } else {
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)words));
+        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<false>, dim3(grid), dim3(kRegionThreads), words, stream, bits, cloud_slots, B,
+                                   K, W, N, keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out,
+                                   static_cast<int*>(workspace)));
+    }
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
 }
 
 extern "C" int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep, const int* keep_count,
                                  const long long* nbr, int k1, int min_area, uint32_t* bits_out, int* area_out, float* score_out,
                                  void* workspace, cudaStream_t stream) {
-    if (!keep_count || !nbr || !workspace) return PSAM_ERR_ARG;
-    if (K > 0 && (!bits || !keep || !bits_out || !area_out || !score_out)) return PSAM_ERR_ARG;
-    if (N <= 0 || N > kRegionMaxN || W < psam::ceil_div(N, 32) || k1 < 1 || k1 > N || K < 0 || K > kNmsMaxK || min_area < 1)
-        return PSAM_ERR_ARG;
-    if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
-    if (K == 0) return PSAM_OK;
-    // persistent grid: two CTAs per SM in the shared-memory form, one per label slice (at most one per SM) otherwise
-    int dev = 0, sms = 0;
-    PSAM_CUDA_TRY(cudaGetDevice(&dev));
-    PSAM_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const int grid = N <= kRegionSmemMaxN ? min(K, 2 * sms) : min(region_slices(K, N), sms);
-    const size_t words = (size_t)(psam::ceil_div(N, 32) + 3) / 4 * 4 * sizeof(uint32_t);
-    if (N <= kRegionSmemMaxN) {
-        const size_t smem = words + (size_t)N * sizeof(int);
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<true>, dim3(grid), dim3(kRegionThreads), smem, stream, bits, K, W, N, keep,
-                                   keep_count, nbr, k1, min_area, bits_out, area_out, score_out, (int*)nullptr));
-    } else {
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)words));
-        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<false>, dim3(grid), dim3(kRegionThreads), words, stream, bits, K, W, N, keep,
-                                   keep_count, nbr, k1, min_area, bits_out, area_out, score_out, static_cast<int*>(workspace)));
-    }
-    PSAM_LAUNCH_CHECK();
-    return PSAM_OK;
+    return psam_mask_regions_batched(bits, 0, 1, K, W, N, keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out,
+                                     workspace, stream);
 }

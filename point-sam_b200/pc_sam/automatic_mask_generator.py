@@ -1,5 +1,5 @@
-"""Automatic mask generation ("segment everything") for one point cloud: the point-cloud counterpart of segment-anything's
-``SamAutomaticMaskGenerator``.
+"""Automatic mask generation ("segment everything") for a point cloud or a batch of clouds: the point-cloud counterpart of
+segment-anything's ``SamAutomaticMaskGenerator``.
 
 1. Encode the cloud once (``model._encode``).
 2. Pick ``points_per_cloud`` prompt points by farthest-point sampling - the point-cloud analogue of SAM's regular grid -
@@ -16,6 +16,11 @@
 Everything runs on the GPU, and the only host synchronisation is the final read of the number of kept masks.  The
 default thresholds are SAM's; they are not tuned for Point-SAM.
 
+Batches of clouds (``generate_packed_batch`` / ``generate_batch``, B clouds of the same N): one encode and one FPS call for
+all B clouds; each decode batch covers the same prompt range of every cloud (``plan_decode``), and every candidate, NMS and
+small-region launch covers all B clouds, each owning a block of ``points_per_cloud * 3`` candidate slots.  One host read
+covers all B kept counts.  Generation on one cloud is the case B = 1 of the same code.
+
 Crop layers (keyword ``crop_n_layers > 0``, SAM's zoomed crops for large scenes): ``psam_crop_layout_f32`` splits the cloud's
 bounding box into 2^i x 2^i x 2^i overlapping boxes on layer i and counts their points; the host reads the counts once.
 Layer 0 runs steps 1-5 on the cloud as given.  Every other crop with at least as many points as the tokenizer's first-level
@@ -25,18 +30,43 @@ touch an interior face of the crop (``psam_crop_edge_filter``).  ``psam_crop_unc
 whole cloud, and ``psam_mask_nms`` with score = layer and ``crop_nms_thresh`` merges them (smaller crops win).  Step 6
 then runs on the merged set.  The host synchronises twice: the counts, and the final read.
 
-Memory: each batch of Z = points_per_batch prompts decodes Z rows of N points.  The split-bf16 input of the last
-upscaling Linear is Z*N*Du*4 bytes (Du = 256 for PointCloudSAM, 128 for PointCloudSAMHier): about 2 GB at Z = 64,
+Memory: each batch of Z = points_per_batch prompts decodes Z rows of N points (with B clouds, points_per_batch // B
+prompts of each cloud).  The split-bf16 input of the last upscaling Linear is Z*N*Du*4 bytes (Du = 256 for PointCloudSAM, 128 for PointCloudSAMHier): about 2 GB at Z = 64,
 N = 32768, Du = 256.  Lower points_per_batch to trade speed for memory.
 """
 from __future__ import annotations
 
-from typing import Dict, List, NamedTuple
+from typing import Dict, List, NamedTuple, Tuple
 
 import numpy as np
 import torch
 
 from psam_b200 import engine, ops
+
+
+# the decoder's upscaling GEMM runs on B * Zc * N rows in tiles of DECODE_ROW_TILE, and its grid holds at most
+# DECODE_MAX_ROW_TILES of them
+DECODE_ROW_TILE, DECODE_MAX_ROW_TILES = 128, 65535
+
+
+class DecodePlan(NamedTuple):
+    rows: int                       # Zc: prompts of each cloud per decode batch
+    batches: List[Tuple[int, int]]  # the prompt range [s, e) of every cloud, one entry per decode batch
+
+
+def plan_decode(B: int, P: int, N: int, points_per_batch: int) -> DecodePlan:
+    """Decode batches for B clouds of N points with P prompts each.  A batch covers prompts [s, e) of every cloud, row
+    b * (e - s) + j of the decoder for prompt s + j of cloud b.  Zc = max(1, points_per_batch // B) keeps points_per_batch
+    rows per batch (the memory bound of the module docstring); the last batch may be short.  Raises ValueError when even
+    one prompt per cloud needs more than DECODE_MAX_ROW_TILES row tiles (ceil(B * N / 128)): fewer clouds per call fit."""
+    if B < 1 or P < 1 or N < 1 or points_per_batch < 1:
+        raise ValueError(f"plan_decode: B, P, N and points_per_batch must be >= 1, got {B}, {P}, {N}, {points_per_batch}")
+    tiles = -(-B * N // DECODE_ROW_TILE)
+    if tiles > DECODE_MAX_ROW_TILES:
+        raise ValueError(f"{B} clouds of {N} points need {tiles} row tiles in the decoder even with one prompt per cloud, at "
+                         f"most {DECODE_MAX_ROW_TILES}: generate fewer clouds per call")
+    Zc = max(1, points_per_batch // B)
+    return DecodePlan(Zc, [(s, min(P, s + Zc)) for s in range(0, P, Zc)])
 
 
 class CropArgs(NamedTuple):
@@ -100,33 +130,62 @@ class PointCloudMaskGenerator:
             raise ValueError(f"{name} must be [N, 3] or [1, N, 3] (one cloud per call), got {tuple(t.shape)}")
         return t.float().contiguous()
 
-    def _generate_one(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None) -> Dict[str, torch.Tensor]:
-        """Generation on one cloud [1, N, 3] (the whole cloud, or one crop's renormalised cloud): encode, P FPS prompts,
-        batched multimask decode, candidates, the crop's edge filter when `edge` is given, mask NMS."""
-        m, dev, N, Bp = self.model, xyz.device, xyz.shape[1], self.points_per_batch
+    @staticmethod
+    def _clouds(t: torch.Tensor, name: str) -> torch.Tensor:
+        if t.dim() != 3 or t.shape[0] < 1 or t.shape[2] != 3:
+            raise ValueError(f"{name} must be [B, N, 3], got {tuple(t.shape)}")
+        return t.float().contiguous()
+
+    @staticmethod
+    def _cloud_state(st: Dict, b: int) -> Dict:
+        """Cloud b of a batched state: every per-cloud tensor indexed by b, the counts kept as one-element tensors."""
+        per_cloud = ("bits", "area", "stability", "score", "keep", "point_index", "centers", "region_bits", "region_area",
+                     "region_score", "region_keep")
+        return {k: (v[b] if k in per_cloud else v[b:b + 1] if k in ("keep_count", "region_count") else v) for k, v in st.items()}
+
+    def _generate_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None) -> Dict[str, torch.Tensor]:
+        """Generation on B clouds [B, N, 3] (whole clouds, or one crop's renormalised cloud, B = 1): one encode, P FPS
+        prompts per cloud, multimask decode in the batches of plan_decode with one candidate launch each, the crop's edge
+        filter when `edge` is given (B = 1), mask NMS per cloud in one go.  Cloud b owns candidate slots b * P * C .. of
+        bits [B, P*C, W]; keep [B, P*C] holds slots within the cloud, keep_count [B]."""
+        m, dev, (B, N, _) = self.model, xyz.device, xyz.shape
+        plan = plan_decode(B, P, N, self.points_per_batch)
         enc = m._encode(xyz, rgb)
         point_index, centers = ops.fps(xyz, P)
-        labels = torch.ones((min(Bp, P), 1), dtype=torch.int64, device=dev)
+        labels = torch.ones((B * plan.rows, 1), dtype=torch.int64, device=dev)
         cand, C = None, None
-        for s in range(0, P, Bp):
-            e = min(P, s + Bp)
-            masks, iou = m._decode_unchecked(enc, centers[0, s:e].unsqueeze(1), labels[: e - s], None, True)
+        for s, e in plan.batches:
+            rows = B * (e - s)
+            masks, iou = m._decode_unchecked(enc, centers[:, s:e].reshape(rows, 1, 3), labels[:rows], None, True)
             if cand is None:
                 C = masks.shape[1]
                 K = P * C
-                cand = (torch.empty((K, ops.mask_words(N)), dtype=torch.int32, device=dev),
-                        torch.empty(K, dtype=torch.int32, device=dev), torch.empty(K, dtype=torch.float32, device=dev),
-                        torch.empty(K, dtype=torch.float32, device=dev))
-            ops.mask_candidates(masks, iou, mask_threshold=self.mask_threshold,
-                                stability_offset=self.stability_score_offset, pred_iou_thresh=self.pred_iou_thresh,
-                                stability_thresh=self.stability_score_thresh, min_area=self.min_mask_area, out=cand,
-                                base=s * C)
+                cand = (torch.empty((B, K, ops.mask_words(N)), dtype=torch.int32, device=dev),
+                        torch.empty((B, K), dtype=torch.int32, device=dev), torch.empty((B, K), dtype=torch.float32, device=dev),
+                        torch.empty((B, K), dtype=torch.float32, device=dev))
+            ops.mask_candidates_batched(masks, iou, B, mask_threshold=self.mask_threshold,
+                                        stability_offset=self.stability_score_offset, pred_iou_thresh=self.pred_iou_thresh,
+                                        stability_thresh=self.stability_score_thresh, min_area=self.min_mask_area, out=cand,
+                                        base=s * C)
         bits, area, stab, score = cand
         if edge is not None:
-            ops.crop_edge_filter(bits, score, edge)
-        keep, keep_count = ops.mask_nms(bits, area, score, self.mask_nms_thresh)
+            ops.crop_edge_filter(bits[0], score[0], edge)
+        keep, keep_count = ops.mask_nms_batched(bits, area, score, self.mask_nms_thresh)
         return dict(bits=bits, area=area, stability=stab, score=score, keep=keep, keep_count=keep_count,
-                    point_index=point_index[0], centers=centers[0], slots=C, device=dev)
+                    point_index=point_index, centers=centers, slots=C, device=dev)
+
+    def _generate_one(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None) -> Dict[str, torch.Tensor]:
+        """_generate_batch on one cloud [1, N, 3], as that cloud's state (bits [K, W], keep [K], keep_count [1], ...)."""
+        return self._cloud_state(self._generate_batch(xyz, rgb, P, edge), 0)
+
+    def _regions(self, xyz: torch.Tensor, bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor,
+                 area: int) -> Dict[str, torch.Tensor]:
+        """The small-region stage on B clouds xyz [B, N, 3]: kept masks keep [B, K] (keep_count [B]) of bits [B, K', W];
+        one kNN launch, one region launch, then mask NMS per cloud in one go."""
+        nbr, _ = ops.knn(xyz, xyz, min(self.region_neighbors + 1, xyz.shape[1]))
+        rbits, rarea, rscore = ops.mask_regions_batched(bits, keep, keep_count, nbr, area)
+        rkeep, rcount = ops.mask_nms_batched(rbits, rarea, rscore, self.mask_nms_thresh)
+        return dict(region_bits=rbits, region_area=rarea, region_score=rscore, region_keep=rkeep, region_count=rcount)
 
     @staticmethod
     def _crop_args(crop_n_layers, crop_nms_thresh, crop_overlap_ratio, crop_n_points_downscale_factor) -> CropArgs:
@@ -190,50 +249,79 @@ class PointCloudMaskGenerator:
                     mask_slot=gslot, crop=gcrop, crop_score=gscore, crop_boxes=boxes, crop_counts=counts, crops=crops,
                     overflow=overflow, lifted_count=offsets[-1:], xyz=xyz[0], device=dev)
 
+    @staticmethod
+    def _region_area(min_mask_region_area: int) -> int:
+        if min_mask_region_area < 0:
+            raise ValueError(f"min_mask_region_area must be >= 0, got {min_mask_region_area}")
+        return int(min_mask_region_area)
+
+    def _check_model(self):
+        if self.model.training:
+            raise NotImplementedError("psam_b200 is an inference-only path: call model.eval() before generating masks")
+
+    @staticmethod
+    def _same_points(xyz: torch.Tensor, rgb: torch.Tensor):
+        if xyz.shape[:2] != rgb.shape[:2]:
+            raise ValueError("xyz and rgb must have the same number of clouds and points")
+
+    def _enqueue_clouds(self, xyz: torch.Tensor, rgb: torch.Tensor, region_area: int) -> Dict[str, torch.Tensor]:
+        """Generation and (region_area > 0) the small-region stage on B validated clouds [B, N, 3], batched state."""
+        with torch.no_grad():
+            st = self._generate_batch(xyz, rgb, min(self.points_per_cloud, xyz.shape[1]))
+            if region_area > 0:
+                st.update(self._regions(xyz, st["bits"], st["keep"], st["keep_count"], region_area))
+        return st
+
     def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
                  crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
                  crop_n_points_downscale_factor: int = 1, keep_crop_states: bool = False) -> Dict[str, torch.Tensor]:
-        """Enqueue the whole generation on the current stream.  Without crop layers nothing here waits for the device; with
-        them, the crop point counts are read once.  keep_crop_states keeps every crop's generation state in st["crops"]
-        (for inspection; it holds each crop's candidate masks until the state is dropped)."""
-        if min_mask_region_area < 0:
-            raise ValueError(f"min_mask_region_area must be >= 0, got {min_mask_region_area}")
+        """Enqueue the whole generation of one cloud on the current stream.  Without crop layers nothing here waits for the
+        device (it is cloud 0 of _enqueue_batch); with them, the crop point counts are read once.  keep_crop_states keeps
+        every crop's generation state in st["crops"] (for inspection; it holds each crop's candidate masks until the state
+        is dropped)."""
+        region_area = self._region_area(min_mask_region_area)
         crop = self._crop_args(crop_n_layers, crop_nms_thresh, crop_overlap_ratio, crop_n_points_downscale_factor)
-        region_area = int(min_mask_region_area)
-        m = self.model
-        if m.training:
-            raise NotImplementedError("psam_b200 is an inference-only path: call model.eval() before generating masks")
+        self._check_model()
         xyz, rgb = self._cloud(xyz, "xyz"), self._cloud(rgb, "rgb")
-        if xyz.shape[1] != rgb.shape[1]:
-            raise ValueError("xyz and rgb must have the same number of points")
-        N = xyz.shape[1]
+        self._same_points(xyz, rgb)
+        if crop.n_layers == 0:
+            return self._cloud_state(self._enqueue_clouds(xyz, rgb, region_area), 0)
         with torch.no_grad():
-            if crop.n_layers > 0:
-                st = self._enqueue_crops(xyz, rgb, crop, keep_crop_states)
-            else:
-                st = self._generate_one(xyz, rgb, min(self.points_per_cloud, N))
+            st = self._enqueue_crops(xyz, rgb, crop, keep_crop_states)
             if region_area > 0:
-                nbr, _ = ops.knn(xyz, xyz, min(self.region_neighbors + 1, N))
-                rbits, rarea, rscore = ops.mask_regions(st["bits"], st["keep"], st["keep_count"], nbr, region_area)
-                rkeep, rcount = ops.mask_nms(rbits, rarea, rscore, self.mask_nms_thresh)
-                st.update(region_bits=rbits, region_area=rarea, region_score=rscore, region_keep=rkeep, region_count=rcount)
+                st.update(self._cloud_state(self._regions(xyz, st["bits"][None], st["keep"][None], st["keep_count"], region_area), 0))
         return st
 
+    def _enqueue_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
+        """Enqueue the generation of B clouds [B, N, 3] on the current stream; nothing here waits for the device."""
+        region_area = self._region_area(min_mask_region_area)
+        self._check_model()
+        xyz, rgb = self._clouds(xyz, "xyz"), self._clouds(rgb, "rgb")
+        self._same_points(xyz, rgb)
+        return self._enqueue_clouds(xyz, rgb, region_area)
+
     @staticmethod
-    def _finish(st: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
-        """The single host synchronisation: read the kept count together with the out-of-range flag of the prompt
-        encoder, then select the kept candidates (on the device).  After the small-region stage the count is the second
-        NMS's, its keep list holds ranks of the first, and bits / area come from the post-processed masks."""
+    def _read_counts(st: Dict[str, torch.Tensor]) -> List[int]:
+        """The single host synchronisation: every cloud's kept count (after the small-region stage, the second NMS's), read
+        together with the out-of-range flag of the prompt encoder and, with crop layers, the overflow flag."""
         flag = engine.bad_flag(st["device"])
-        regions, crops = "region_keep" in st, "crops" in st
-        reads = [st["region_count" if regions else "keep_count"], flag] + ([st["overflow"]] if crops else [])
-        n, bad, *over = (int(v) for v in torch.cat(reads).tolist())
-        if bad:
+        counts = st["region_count" if "region_keep" in st else "keep_count"]
+        crops = "crops" in st
+        vals = [int(v) for v in torch.cat([counts, flag] + ([st["overflow"]] if crops else [])).tolist()]
+        B = counts.numel()
+        if vals[B]:
             flag.zero_()
             raise ValueError("Input coordinates must be normalized to [-1, 1].")
-        if over and over[0]:
+        if crops and vals[B + 1]:
             raise ValueError(f"crop layers: the kept masks of all crops exceed the {st['bits'].shape[0]} lifted slots; "
                              "lower points_per_cloud or crop_n_layers, or raise crop_n_points_downscale_factor")
+        return vals[:B]
+
+    @staticmethod
+    def _select(st: Dict[str, torch.Tensor], n: int) -> Dict[str, torch.Tensor]:
+        """The n kept masks of one cloud's state, selected on the device.  After the small-region stage the keep list is the
+        second NMS's and holds ranks of the first, and bits / area come from the post-processed masks."""
+        regions, crops = "region_keep" in st, "crops" in st
         if regions:
             rank = st["region_keep"][:n].long()
             sel = st["keep"][rank].long()
@@ -250,6 +338,17 @@ class PointCloudMaskGenerator:
         return dict(bits=bits, area=area, predicted_iou=st["score"][sel],
                     stability_score=st["stability"][sel], point_index=st["point_index"][z], point_coords=st["centers"][z],
                     mask_slot=sel - z * st["slots"])
+
+    @classmethod
+    def _finish(cls, st: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """One cloud's output from its state (_enqueue), after the single host synchronisation."""
+        (n,) = cls._read_counts(st)
+        return cls._select(st, n)
+
+    @classmethod
+    def _finish_batch(cls, st: Dict[str, torch.Tensor]) -> List[Dict[str, torch.Tensor]]:
+        """Every cloud's output from a batched state (_enqueue_batch), after one host synchronisation for all of them."""
+        return [cls._select(cls._cloud_state(st, b), n) for b, n in enumerate(cls._read_counts(st))]
 
     def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
                         crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
@@ -275,16 +374,17 @@ class PointCloudMaskGenerator:
                                           crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
                                           crop_n_points_downscale_factor=crop_n_points_downscale_factor))
 
-    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
-                 crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
-                 crop_n_points_downscale_factor: int = 1) -> List[Dict]:
-        """SAM's record list, in the order of generate_packed: segmentation (bool [N] numpy), area, predicted_iou,
-        stability_score, point_coords ([[x, y, z]]), point_index, and crop_box ([x0, y0, z0, x1, y1, z1]) with crop
-        layers."""
-        N = self._cloud(xyz, "xyz").shape[1]
-        out = self.generate_packed(xyz, rgb, min_mask_region_area=min_mask_region_area, crop_n_layers=crop_n_layers,
-                                   crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
-                                   crop_n_points_downscale_factor=crop_n_points_downscale_factor)
+    def generate_packed_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *,
+                              min_mask_region_area: int = 0) -> List[Dict[str, torch.Tensor]]:
+        """generate_packed on B clouds of the same N at once: xyz / rgb [B, N, 3] CUDA tensors, xyz normalised to [-1, 1].
+        Returns B dicts with generate_packed's fields, dtypes, order and meaning for each cloud.  The clouds share one encode,
+        the decode batches (points_per_batch // B prompts of every cloud each) and every post-processing launch, and the host
+        synchronises once for all of them; a cloud outside [-1, 1] raises ValueError for the whole call.  Crop layers are
+        not supported here (crops of different clouds differ in size): use generate_packed per cloud."""
+        return self._finish_batch(self._enqueue_batch(xyz, rgb, min_mask_region_area=min_mask_region_area))
+
+    @staticmethod
+    def _records(out: Dict[str, torch.Tensor], N: int) -> List[Dict]:
         out = {k: v.cpu().numpy() for k, v in out.items()}
         seg = np.unpackbits(out["bits"].astype("<i4").view(np.uint8), axis=1, bitorder="little")[:, :N].astype(bool)
         recs = [dict(segmentation=seg[i], area=int(out["area"][i]), predicted_iou=float(out["predicted_iou"][i]),
@@ -294,3 +394,19 @@ class PointCloudMaskGenerator:
             for r, box in zip(recs, out["crop_box"]):
                 r["crop_box"] = box.tolist()
         return recs
+
+    def generate(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
+                 crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
+                 crop_n_points_downscale_factor: int = 1) -> List[Dict]:
+        """SAM's record list, in the order of generate_packed: segmentation (bool [N] numpy), area, predicted_iou,
+        stability_score, point_coords ([[x, y, z]]), point_index, and crop_box ([x0, y0, z0, x1, y1, z1]) with crop
+        layers."""
+        N = self._cloud(xyz, "xyz").shape[1]
+        return self._records(self.generate_packed(xyz, rgb, min_mask_region_area=min_mask_region_area, crop_n_layers=crop_n_layers,
+                                                  crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
+                                                  crop_n_points_downscale_factor=crop_n_points_downscale_factor), N)
+
+    def generate_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> List[List[Dict]]:
+        """generate on B clouds [B, N, 3] at once (see generate_packed_batch): one record list per cloud."""
+        N = self._clouds(xyz, "xyz").shape[1]
+        return [self._records(out, N) for out in self.generate_packed_batch(xyz, rgb, min_mask_region_area=min_mask_region_area)]

@@ -64,6 +64,8 @@ EXPORTS = [
     "psam_decoder_prepare", "psam_interp_ln_gelu", "psam_interp_add_ln_gelu", "psam_mask_dot", "psam_add_bcast_f32", "psam_split_f32", "psam_split_add_f32",
     "psam_mask_candidates_f32", "psam_mask_nms_workspace_bytes", "psam_mask_nms",
     "psam_mask_regions_workspace_bytes", "psam_mask_regions",
+    "psam_mask_candidates_batched_f32", "psam_mask_nms_batched_workspace_bytes", "psam_mask_nms_batched",
+    "psam_mask_regions_batched_workspace_bytes", "psam_mask_regions_batched",
     "psam_crop_total", "psam_crop_layout_f32", "psam_crop_gather_workspace_bytes", "psam_crop_gather_f32", "psam_crop_edge_filter",
     "psam_crop_uncrop",
     "psam_version",
@@ -88,6 +90,10 @@ def lib():
         L.psam_mask_nms_workspace_bytes.argtypes = [i, i]
         L.psam_mask_regions_workspace_bytes.restype = c_size_t
         L.psam_mask_regions_workspace_bytes.argtypes = [i, i]
+        L.psam_mask_nms_batched_workspace_bytes.restype = c_size_t
+        L.psam_mask_nms_batched_workspace_bytes.argtypes = [i, i, i]
+        L.psam_mask_regions_batched_workspace_bytes.restype = c_size_t
+        L.psam_mask_regions_batched_workspace_bytes.argtypes = [i, i, i]
         L.psam_crop_gather_workspace_bytes.restype = c_size_t
         L.psam_crop_gather_workspace_bytes.argtypes = [i]
         sig = {
@@ -122,6 +128,9 @@ def lib():
             "psam_mask_candidates_f32": [p, p, i, i, i, f, f, f, f, i, ll, i, p, p, p, p, p],
             "psam_mask_nms": [p, p, p, i, i, f, p, p, p, p],
             "psam_mask_regions": [p, i, i, i, p, p, p, i, i, p, p, p, p, p],
+            "psam_mask_candidates_batched_f32": [p, p, i, i, i, i, f, f, f, f, i, ll, ll, i, p, p, p, p, p],
+            "psam_mask_nms_batched": [p, p, p, i, i, i, f, p, p, p, p],
+            "psam_mask_regions_batched": [p, ll, i, i, i, i, p, p, p, i, i, p, p, p, p, p],
             "psam_crop_total": [i],
             "psam_crop_layout_f32": [p, i, i, f, p, p, p],
             "psam_crop_gather_f32": [p, p, i, p, i, i, f, i, p, p, p, p, p, p],

@@ -403,6 +403,68 @@ def mask_regions(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tenso
     return bits_out, area_out, score_out
 
 
+def mask_candidates_batched(logits: torch.Tensor, iou_preds: torch.Tensor, B: int, *, out, base: int = 0,
+                            mask_threshold: float = 0.0, stability_offset: float = 1.0, pred_iou_thresh: float = 0.0,
+                            stability_thresh: float = 0.0, min_area: int = 0):
+    """mask_candidates for B clouds in one launch (psam_mask_candidates_batched_f32): logits [B*Zc,C,N], iou_preds [B*Zc,C],
+    rows b*Zc .. b*Zc+Zc-1 of cloud b.  Row b*Zc + j, output c fills slot base + j*C + c of cloud b in
+    out = (bits [B,K,W] int32, area [B,K] int32, stability [B,K] fp32, score [B,K] fp32)."""
+    Z, C, N = logits.shape
+    bits, area, stab, score = out
+    if B < 1 or Z % B or bits.shape[0] != B:
+        raise ValueError(f"mask_candidates_batched: {Z} rows and {bits.shape[0]} candidate blocks for {B} clouds")
+    Zc, K = Z // B, bits.shape[1]
+    if base < 0 or base + Zc * C > K:
+        raise ValueError(f"mask_candidates_batched: slots {base}..{base + Zc * C} do not fit {K} candidates per cloud")
+    lg = logits.float().contiguous()
+    io = iou_preds.float().contiguous()
+    nv.check(nv.lib().psam_mask_candidates_batched_f32(nv.ptr(lg), nv.ptr(io), B, Zc, C, N, float(mask_threshold),
+                                                       float(stability_offset), float(pred_iou_thresh), float(stability_thresh),
+                                                       int(min_area), int(base), K, bits.shape[2], nv.ptr(bits), nv.ptr(area),
+                                                       nv.ptr(stab), nv.ptr(score), nv.stream()), "mask_candidates_batched")
+    return out
+
+
+def mask_nms_batched(bits: torch.Tensor, area: torch.Tensor, score: torch.Tensor, nms_thresh: float):
+    """mask_nms on each of B clouds in the same three launches (psam_mask_nms_batched): bits [B,K,W], area / score [B,K].
+    Returns (keep [B, max(K,1)] int32: each cloud's kept slots 0..K-1 in score order, keep_count [B] int32), on the device."""
+    B, K, W = bits.shape
+    if K > NMS_MAX_CANDIDATES:
+        raise ValueError(f"mask_nms_batched: {K} candidates per cloud, at most {NMS_MAX_CANDIDATES}")
+    dev = bits.device
+    keep = torch.empty((B, max(K, 1)), dtype=torch.int32, device=dev)
+    keep_count = torch.empty(B, dtype=torch.int32, device=dev)
+    ws = torch.empty(nv.lib().psam_mask_nms_batched_workspace_bytes(B, K, W), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_mask_nms_batched(nv.ptr(bits) if K else None, nv.ptr(area) if K else None, nv.ptr(score) if K else None,
+                                            B, K, W, float(nms_thresh), nv.ptr(keep), nv.ptr(keep_count), nv.ptr(ws), nv.stream()),
+             "mask_nms_batched")
+    return keep, keep_count
+
+
+def mask_regions_batched(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor, nbr: torch.Tensor, min_area: int):
+    """mask_regions on each of B clouds in one launch (psam_mask_regions_batched): candidate masks bits [B,K',W], kept slots
+    keep [B,K] with counts keep_count [B], kNN graphs nbr [B,N,k1].  Returns (bits_out [B,K,W], area_out [B,K],
+    score_out [B,K]) by kept rank; nothing waits for the device."""
+    B, Kc, W = bits.shape
+    K = keep.shape[1]
+    N, k1 = nbr.shape[-2], nbr.shape[-1]
+    if keep.shape[0] != B or keep_count.numel() != B or nbr.shape[0] != B:
+        raise ValueError(f"mask_regions_batched: keep {tuple(keep.shape)}, keep_count {tuple(keep_count.shape)} and nbr "
+                         f"{tuple(nbr.shape)} do not match {B} clouds")
+    if K > NMS_MAX_CANDIDATES:
+        raise ValueError(f"mask_regions_batched: {K} kept masks per cloud, at most {NMS_MAX_CANDIDATES}")
+    keep, nbr = keep.contiguous(), nbr.contiguous()
+    dev = bits.device
+    bits_out = torch.empty((B, K, W), dtype=torch.int32, device=dev)
+    area_out = torch.empty((B, K), dtype=torch.int32, device=dev)
+    score_out = torch.empty((B, K), dtype=torch.float32, device=dev)
+    ws = torch.empty(nv.lib().psam_mask_regions_batched_workspace_bytes(B, K, N), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_mask_regions_batched(nv.ptr(bits), Kc, B, K, W, N, nv.ptr(keep), nv.ptr(keep_count), nv.ptr(nbr), k1,
+                                                int(min_area), nv.ptr(bits_out), nv.ptr(area_out), nv.ptr(score_out), nv.ptr(ws),
+                                                nv.stream()), "mask_regions_batched")
+    return bits_out, area_out, score_out
+
+
 # ------------------------------------------------------------------------------------------------
 # crop layers of automatic mask generation
 # ------------------------------------------------------------------------------------------------
