@@ -453,6 +453,58 @@ int psam_crop_uncrop(const uint32_t* bits, const int* area, const float* score, 
                      uint32_t* gbits, int* garea, float* giou, float* gstab, long long* gprompt, int* gslot, int* gcrop,
                      float* gscore, int* overflow, cudaStream_t stream);
 
+/* ---- meshes and dense clouds ---------------------------------------------------------------------- */
+/* Area-weighted surface sampling of a triangle mesh: vertices [V, 3] fp32, faces [F, 3] int32 -> S samples xyz_out [S, 3],
+ * rgb_out [S, 3] and face_out [S] (int32, the face each sample lies on).  Everything is fp32, every operation rounded on its
+ * own (no contraction), in this order, unless stated otherwise:
+ *   weight  e1 = b - a, e2 = c - a (a, b, c = the face's vertices), n = (e1y*e2z - e1z*e2y, e1z*e2x - e1x*e2z,
+ *           e1x*e2y - e1y*e2x), A2 = sqrt((nx*nx + ny*ny) + nz*nz) (twice the area).  A face with an index outside [0, V),
+ *           or whose A2 is not finite or <= 0, has weight 0 (a "bad" face).  With A2max in [2^(E-1), 2^E) the largest A2 of
+ *           the good faces, the weight is the integer q_f = floor(A2_f * 2^(32 - E)) (computed in fp64, where it is exact),
+ *           so q_f <= 2^32 - 1, and a face smaller than 2^-32 of the largest has weight 0 and is never sampled.
+ *   cdf     cdf[f] = q_0 + ... + q_f, an exact uint64 prefix sum; total = cdf[F - 1].
+ *   hash    h_j(s) = splitmix64 finaliser of seed + (3*s + j + 1) * 0x9E3779B97F4A7C15 (mod 2^64), streams j = 0, 1, 2 of
+ *           sample s: z ^= z >> 30, z *= 0xBF58476D1CE4E5B9, z ^= z >> 27, z *= 0x94D049BB133111EB, z ^= z >> 31.  There is no
+ *           generator state, so the samples do not depend on the launch configuration.
+ *   face    u = mulhi64(h_0, total) (the high 64 bits of the 128-bit product); the face is the smallest f with cdf[f] > u, so
+ *           a face is chosen with probability q_f / total and a weight-0 face never.
+ *   point   r1 = (h_1 >> 40) * 2^-24, r2 = (h_2 >> 40) * 2^-24 (exact), v = sqrt(r1), w = (1 - v, v * (1 - r2), v * r2);
+ *           p = (w0 * a + w1 * b) + w2 * c, then each axis clamped to [min, max] of the three vertices' coordinates (so the
+ *           samples of a mesh inside [-1, 1] stay inside it).
+ *   colour  with texture [tex_h, tex_w, tex_c] uint8 (tex_c = 3 or 4) and uv [V, 2]: (tu, tv) = the uv interpolated like p
+ *           (not clamped), texel x = floor(tu * tex_w + 0.5), y = floor((1 - tv) * tex_h + 0.5), each clamped into the image
+ *           (a NaN gives 0); the colour is its first three channels / 255.  Otherwise with vertex_colors [V, 3]: interpolated
+ *           and clamped like p.  With neither: 0.5.  texture and vertex_colors are exclusive; uv goes with texture.
+ * stats (device int64 [3]): stats[0] = total weight, stats[1] = bad faces, stats[2] = faces with an index outside [0, V)
+ * (counted among the bad faces).  When the total weight is 0 every sample gets face -1, xyz 0 and rgb 0.
+ * Five launches (areas, three for the scan, samples) and two memsets, no host synchronisation.  1 <= V, 1 <= F < 2^31,
+ * 1 <= S.  workspace: psam_mesh_sample_workspace_bytes(F) bytes, 16-byte aligned.  Bad arguments -> PSAM_ERR_ARG before any
+ * CUDA call. */
+size_t psam_mesh_sample_workspace_bytes(int F);
+int psam_mesh_sample_f32(const float* vertices, int V, const int* faces, int F, int S, unsigned long long seed,
+                         const float* vertex_colors, const float* uv, const unsigned char* texture, int tex_h, int tex_w, int tex_c,
+                         float* xyz_out, float* rgb_out, int* face_out, long long* stats, void* workspace, cudaStream_t stream);
+
+/* centers[f] = ((a + b) + c) / 3 per axis in fp32 (IEEE division), NaN for a face with an index outside [0, V): the query
+ * points that carry masks to faces (psam_nn_distance_f32 gives such a query no nearest sample, index -1).
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mesh_face_centers_f32(const float* vertices, int V, const int* faces, int F, float* centers, cudaStream_t stream);
+
+/* Mask lifting: masks over S points carried to M other points through their nearest point.  bits [K, Ws] (bit-packed as in
+ * psam_mask_candidates_f32, Ws >= ceil(S/32)), nearest [M] int64 -> bits_out [K, Wm] (Wm >= ceil(M/32)): bit t of row k is
+ * bit nearest[t] of row k of bits; an entry outside [0, S) reads as 0, and bits past M and words past ceil(M/32) are 0.
+ * area_out[k] = the number of set bits of row k of bits_out (exact).  Two launches: one warp per 4 output words, each lane
+ * holding its nearest index across all K rows, then one warp per row for the areas.  K = 0 is a no-op (pointers may be
+ * NULL).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_lift(const uint32_t* bits, int K, int Ws, int S, const long long* nearest, int M, int Wm, uint32_t* bits_out,
+                   int* area_out, cudaStream_t stream);
+
+/* Part labels: labels[n] = the row k of bits [K, W] (W >= ceil(N/32)) that contains point n with the smallest priority[k]
+ * (int32), ties to the lower k; -1 when no row contains it.  With priority = area the smallest mask containing a point wins,
+ * which is the order in which segment-anything's show_anns paints (largest first, so the smallest ends on top).  K = 0 gives
+ * -1 everywhere.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_label_map(const uint32_t* bits, int K, int W, const int* priority, int N, int* labels, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

@@ -68,6 +68,7 @@ EXPORTS = [
     "psam_mask_regions_batched_workspace_bytes", "psam_mask_regions_batched",
     "psam_crop_total", "psam_crop_layout_f32", "psam_crop_gather_workspace_bytes", "psam_crop_gather_f32", "psam_crop_edge_filter",
     "psam_crop_uncrop",
+    "psam_mesh_sample_workspace_bytes", "psam_mesh_sample_f32", "psam_mesh_face_centers_f32", "psam_mask_lift", "psam_mask_label_map",
     "psam_version",
 ]
 
@@ -96,6 +97,8 @@ def lib():
         L.psam_mask_regions_batched_workspace_bytes.argtypes = [i, i, i]
         L.psam_crop_gather_workspace_bytes.restype = c_size_t
         L.psam_crop_gather_workspace_bytes.argtypes = [i]
+        L.psam_mesh_sample_workspace_bytes.restype = c_size_t
+        L.psam_mesh_sample_workspace_bytes.argtypes = [i]
         sig = {
             "psam_fps_f32": [p, i, i, i, p, p, p, p],
             "psam_knn_f32": [p, p, i, i, i, i, p, p, p],
@@ -136,6 +139,10 @@ def lib():
             "psam_crop_gather_f32": [p, p, i, p, i, i, f, i, p, p, p, p, p, p],
             "psam_crop_edge_filter": [p, i, i, p, p, p],
             "psam_crop_uncrop": [p, p, p, p, i, i, p, p, p, i, p, i, i, f, i, i, i, p, p, p, p, p, p, p, p, p, p, p, p],
+            "psam_mesh_sample_f32": [p, i, p, i, i, ctypes.c_uint64, p, p, p, i, i, i, p, p, p, p, p, p],
+            "psam_mesh_face_centers_f32": [p, i, p, i, p, p],
+            "psam_mask_lift": [p, i, i, i, p, i, i, p, p, p],
+            "psam_mask_label_map": [p, i, i, p, i, p, p],
         }
         for name, args in sig.items():
             fn = getattr(L, name)

@@ -530,3 +530,70 @@ def crop_uncrop(cand, keep: torch.Tensor, keep_count: torch.Tensor, idx: torch.T
                                        float(layer_score), int(N), Wg, cap, nv.ptr(offsets[k:]), nv.ptr(offsets[k + 1:]), nv.ptr(gbits),
                                        nv.ptr(garea), nv.ptr(giou), nv.ptr(gstab), nv.ptr(gprompt), nv.ptr(gslot), nv.ptr(gcrop),
                                        nv.ptr(gscore), nv.ptr(overflow), nv.stream()), "crop_uncrop")
+
+
+# ------------------------------------------------------------------------------------------------
+# meshes and dense clouds
+# ------------------------------------------------------------------------------------------------
+def mesh_sample(vertices: torch.Tensor, faces: torch.Tensor, S: int, seed: int = 0, vertex_colors=None, uv=None, texture=None):
+    """S area-weighted samples of a triangle mesh (psam_mesh_sample_f32): vertices [V, 3] fp32, faces [F, 3] int32, optional
+    vertex_colors [V, 3] fp32, or uv [V, 2] fp32 with texture [H, W, C] uint8 (C = 3 or 4).  Returns (xyz [S, 3], rgb [S, 3],
+    face [S] int32, stats [3] int64 = (total weight, bad faces, faces with an index outside [0, V))), all on the device;
+    nothing waits for it."""
+    v = vertices.reshape(-1, 3).float().contiguous()
+    f = faces.reshape(-1, 3).to(torch.int32).contiguous()
+    V, F, dev = v.shape[0], f.shape[0], v.device
+    vc = vertex_colors.reshape(V, 3).float().contiguous() if vertex_colors is not None else None
+    tuv = uv.reshape(V, 2).float().contiguous() if uv is not None else None
+    tex = texture.contiguous() if texture is not None else None
+    if tex is not None and (tex.dim() != 3 or tex.dtype != torch.uint8):
+        raise ValueError(f"mesh_sample: texture must be uint8 [H, W, C], got {tex.dtype} {tuple(tex.shape)}")
+    H, W, C = tuple(tex.shape) if tex is not None else (0, 0, 0)
+    xyz = torch.empty((S, 3), dtype=torch.float32, device=dev)
+    rgb = torch.empty((S, 3), dtype=torch.float32, device=dev)
+    face = torch.empty(S, dtype=torch.int32, device=dev)
+    stats = torch.empty(3, dtype=torch.int64, device=dev)
+    ws = torch.empty(nv.lib().psam_mesh_sample_workspace_bytes(F), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_mesh_sample_f32(nv.ptr(v), V, nv.ptr(f), F, int(S), int(seed) & (2 ** 64 - 1), nv.ptr(vc), nv.ptr(tuv),
+                                           nv.ptr(tex), H, W, C, nv.ptr(xyz), nv.ptr(rgb), nv.ptr(face), nv.ptr(stats), nv.ptr(ws),
+                                           nv.stream()), "mesh_sample")
+    return xyz, rgb, face, stats
+
+
+def mesh_face_centers(vertices: torch.Tensor, faces: torch.Tensor) -> torch.Tensor:
+    """((a + b) + c) / 3 of every face (psam_mesh_face_centers_f32): [F, 3] fp32, NaN for a face with a bad index."""
+    v = vertices.reshape(-1, 3).float().contiguous()
+    f = faces.reshape(-1, 3).to(torch.int32).contiguous()
+    centers = torch.empty((f.shape[0], 3), dtype=torch.float32, device=v.device)
+    nv.check(nv.lib().psam_mesh_face_centers_f32(nv.ptr(v), v.shape[0], nv.ptr(f), f.shape[0], nv.ptr(centers), nv.stream()),
+             "mesh_face_centers")
+    return centers
+
+
+def mask_lift(bits: torch.Tensor, nearest: torch.Tensor, S: int):
+    """Masks over S points carried to M points through their nearest point (psam_mask_lift): bits [K, W >= mask_words(S)]
+    int32, nearest [M] int64 (entries outside [0, S) read as 0).  Returns (bits [K, mask_words(M)] int32, area [K] int32)."""
+    K, Ws = bits.shape
+    near = nearest.reshape(-1).to(torch.int64).contiguous()
+    M, dev = near.shape[0], bits.device
+    Wm = mask_words(M)
+    out = torch.empty((K, Wm), dtype=torch.int32, device=dev)
+    area = torch.empty(K, dtype=torch.int32, device=dev)
+    b = bits.contiguous()
+    nv.check(nv.lib().psam_mask_lift(nv.ptr(b) if K else None, K, Ws, int(S), nv.ptr(near), M, Wm, nv.ptr(out) if K else None,
+                                     nv.ptr(area) if K else None, nv.stream()), "mask_lift")
+    return out, area
+
+
+def mask_label_map(bits: torch.Tensor, priority: torch.Tensor, N: int) -> torch.Tensor:
+    """One label per point (psam_mask_label_map): the row of bits [K, W >= mask_words(N)] containing the point with the
+    smallest priority [K] (int32), ties to the lower row, -1 for a point in no row.  Returns labels [N] int32."""
+    K, W = bits.shape
+    pr = priority.reshape(-1).to(torch.int32).contiguous()
+    if pr.shape[0] != K:
+        raise ValueError(f"mask_label_map: {pr.shape[0]} priorities for {K} masks")
+    labels = torch.empty(int(N), dtype=torch.int32, device=bits.device)
+    b = bits.contiguous()
+    nv.check(nv.lib().psam_mask_label_map(nv.ptr(b) if K else None, K, W, nv.ptr(pr) if K else None, int(N), nv.ptr(labels),
+                                          nv.stream()), "mask_label_map")
+    return labels

@@ -46,3 +46,63 @@ def make_region_masks(xyz: torch.Tensor, num_masks: int = 1) -> torch.Tensor:
     B, N, _ = xyz.shape
     return torch.stack([torch.stack([(xyz[b] - xyz[b, (997 * (m + 1)) % N]).norm(dim=-1) < 0.45 + 0.05 * m
                                      for m in range(num_masks)]) for b in range(B)])
+
+
+def make_sphere(n_lat: int, n_lon: int, center=(0.0, 0.0, 0.0), radius: float = 1.0):
+    """A closed UV sphere: (vertices [2 + (n_lat - 1) n_lon, 3] float32, faces [2 n_lon (n_lat - 1), 3] int32)."""
+    import numpy as np
+
+    th = np.linspace(0, np.pi, n_lat + 1)[1:-1]
+    ph = np.linspace(0, 2 * np.pi, n_lon, endpoint=False)
+    ring = np.stack([np.outer(np.sin(th), np.cos(ph)), np.outer(np.sin(th), np.sin(ph)), np.repeat(np.cos(th)[:, None], n_lon, 1)], -1)
+    v = np.concatenate([[[0, 0, 1]], ring.reshape(-1, 3), [[0, 0, -1]]]) * radius + np.asarray(center)
+    i, j = np.meshgrid(np.arange(n_lat - 2), np.arange(n_lon), indexing="ij")
+    r = lambda i, j: 1 + i * n_lon + j % n_lon  # noqa: E731
+    band = np.stack([np.stack([r(i, j), r(i + 1, j), r(i + 1, j + 1)], -1), np.stack([r(i, j), r(i + 1, j + 1), r(i, j + 1)], -1)], 2)
+    jj = np.arange(n_lon)
+    last = len(v) - 1
+    cap0 = np.stack([np.zeros(n_lon, int), r(0, jj), r(0, jj + 1)], -1)
+    cap1 = np.stack([r(n_lat - 2, jj), np.full(n_lon, last), r(n_lat - 2, jj + 1)], -1)
+    f = np.concatenate([cap0, band.reshape(-1, 3), cap1])
+    return v.astype(np.float32), f.astype(np.int32)
+
+
+def make_box(n: int, center=(0.0, 0.0, 0.0), half=(1.0, 1.0, 1.0)):
+    """The surface of an axis-aligned box, each side an n x n grid of quads split in two: 12 n^2 faces (the sides do not share
+    their edge vertices)."""
+    import numpy as np
+
+    t = np.linspace(-1, 1, n + 1)
+    a, b = np.meshgrid(t, t, indexing="ij")
+    q = np.arange((n + 1) ** 2).reshape(n + 1, n + 1)
+    quad = np.stack([q[:-1, :-1], q[1:, :-1], q[1:, 1:], q[:-1, 1:]], -1).reshape(-1, 4)
+    tri = np.concatenate([quad[:, [0, 1, 2]], quad[:, [0, 2, 3]]])
+    vs, fs = [], []
+    for axis in range(3):
+        for side in (-1.0, 1.0):
+            p = np.zeros(((n + 1) ** 2, 3))
+            u, w = [k for k in range(3) if k != axis]
+            p[:, axis], p[:, u], p[:, w] = side, a.ravel(), b.ravel()
+            fs.append((tri if side > 0 else tri[:, ::-1]) + sum(len(x) for x in vs))
+            vs.append(p)
+    v = np.concatenate(vs) * np.asarray(half) + np.asarray(center)
+    return v.astype(np.float32), np.concatenate(fs).astype(np.int32)
+
+
+def make_mesh(num_faces: int, seed: int = 0):
+    """A scene of four spheres and four boxes of random sizes and positions with about num_faces faces in all:
+    (vertices float32, faces int32, vertex_colors float32 in 0..1, one colour per object)."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+    k = max(3, int(round((num_faces / 16) ** 0.5)))   # a sphere of k x k has about 2 k^2 faces
+    n = max(1, int(round((num_faces / 96) ** 0.5)))    # a box of n has 12 n^2 faces
+    vs, fs, cs, base = [], [], [], 0
+    for o in range(8):
+        c = rng.uniform(-2, 2, 3)
+        v, f = make_sphere(k, k, c, rng.uniform(0.3, 1.0)) if o % 2 == 0 else make_box(n, c, rng.uniform(0.2, 0.8, 3))
+        vs.append(v)
+        fs.append(f + base)
+        cs.append(np.tile(rng.uniform(0, 1, 3), (len(v), 1)))
+        base += len(v)
+    return np.concatenate(vs), np.concatenate(fs), np.concatenate(cs).astype(np.float32)
