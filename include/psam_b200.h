@@ -505,6 +505,72 @@ int psam_mask_lift(const uint32_t* bits, int K, int Ws, int S, const long long* 
  * -1 everywhere.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
 int psam_mask_label_map(const uint32_t* bits, int K, int W, const int* priority, int N, int* labels, cudaStream_t stream);
 
+/* ---- dense scans ---------------------------------------------------------------------------------- */
+/* Exact nearest key on a uniform grid: query [n1, 3], key [n2, 3] -> dist_out [n1] fp32 and idx_out [n1] int64 (may be NULL),
+ * bit for bit what psam_nn_distance_f32 writes for every input:
+ *   d(j) = fma(dz, dz, fma(dy, dy, dx * dx)) with dx = key_x - query_x etc. (each step rounded once);
+ *   the result is the lexicographic minimum of (d(j), j) over the keys with d(j) < 3.4e38f, or (3.4e38f, -1) when there is
+ *   none: so a query with a non-finite coordinate, or whose every distance overflows or is NaN, gets index -1, and a key with
+ *   a non-finite coordinate is never chosen.  Candidates are compared as (d, j) pairs, so the order of the visits is free.
+ * Evaluation order (each call builds the grid afresh over the finite keys, a counting sort):
+ *   box      klo_a / hi_a = min / max of the finite keys' coordinates (exact), F = the number of finite keys, and a
+ *            1024-bin histogram of them on each axis over [klo_a, hi_a].
+ *   grid     its box on axis a runs from lo_a = max(klo_a, b5 - w / 10) to min(hi_a, b95 + w / 10), where b5 is the lower edge
+ *            of the bin holding the key of rank F / 20, b95 the upper edge of the bin holding rank F - 1 - F / 20 and
+ *            w = b95 - b5, so far outliers do not stretch it; T = min(F, 2^22) target cells; cubic cells of side h, with
+ *            dims_a = min(floor(ext_a / h) + 1, 2^21) cells on axis a (ext_a = the box's extent, fp64) and h the (fp64
+ *            bisection) smallest found with dims_x dims_y dims_z <= T; one cell of side 1 when every ext_a is 0.  Keys
+ *            outside the box land in its border cells (the clamp below).  The box, h and the dims decide only the speed.
+ *   cell     c_a(p) = clamp(floor((p_a - lo_a) * (1 / h)), 0, dims_a - 1) in fp64, cell id (c_x dims_y + c_y) dims_z + c_z;
+ *            a histogram (the rank of a key in its cell comes from the counting atomic), an exclusive scan of the counts
+ *            and a scatter of (x, y, z, j) into cell order (the order inside a cell is free).
+ *   search   every query visits the rings r = 0, 1, ... of cells at Chebyshev index distance r from its clamped cell c(q),
+ *            each grid row along z as one contiguous run, and after ring r stops when a lower bound LB on the squared
+ *            distance to every key in an unvisited cell satisfies LB' = LB (1 - 2^-20) - 2^-140 > best d (fp64 compare),
+ *            or LB' >= 3.4e38, or no cell is left.
+ * The lower bound and its margin.  Unvisited cells lie beyond one of the six faces of the visited block (cells c(q)_a - r ..
+ * c(q)_a + r); for the face on axis a at f = lo_a + k h, LB = max(t^2, o_a^2) + sum_{b != a} o_b^2, where o_b = the distance
+ * from q_b to [klo_b, hi_b] (every finite key lies in that box) and t = max(|q_a - f| - s_a, 0) on the face's far side.
+ * The slop s_a = 2^-40 (|lo_a| + |klo_a| + |hi_a| + |q_a| + (dims_a + 1) h) covers the fp64 rounding of the cell coordinates
+ * and of f: a key in cell k >= 1 has (p_a - lo_a)(1 + e1)(1 / h)(1 + e2) >= k with |e1|, |e2| <= 2^-53, so p_a >= f - 2^-50 k h,
+ * and likewise below.  The clamp into the border cells only moves a key into a cell on the same side of every face, so
+ * the bound holds for clamped keys too.  Then, for every unvisited key, its true squared distance D >= LB up to the relative fp64
+ * rounding of LB (a few 2^-53).  Its computed d is five roundings away from D: the subtractions (exact when the result is
+ * subnormal, else relative error <= 2^-24), the product and the two fmas (relative error <= 2^-24, or absolute <= 2^-150
+ * where the result is subnormal).  Every step is monotone, so d >= D (1 - 2^-24)^5 - 3 * 2^-150 >= D (1 - 2^-21) - 2^-148;
+ * a step that overflows gives inf, which is still >= that bound.  Hence d >= LB' for every unvisited key, and LB' > best d
+ * means no unvisited key can win (nor tie with a lower index); LB' >= 3.4e38 means none can be accepted.  A query far
+ * outside the keys' box is answered exactly, by visiting more rings.
+ * Launches: box, box histograms, setup (one thread), cell histogram, one to three for the scan, scatter, queries (one
+ * thread per query, an outward ring search) - up to nine launches after one memset, no host synchronisation.
+ * 1 <= n1 <= 2^31 - 1, 1 <= n2 <= 2^31 - 1.  workspace: psam_nn_grid_workspace_bytes(n2), about 12.4 KB + 4 (C + 1) +
+ * 8 ceil((C + 1) / 1024) + 24 n2 bytes (each part rounded up to 16 bytes) with C = min(n2, 2^22) cells, 16-byte aligned.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_nn_grid_workspace_bytes(int n2);
+int psam_nn_grid_f32(const float* query, int n1, const float* key, int n2, float* dist_out, long long* idx_out, void* workspace,
+                     cudaStream_t stream);
+
+/* Voxel subsample of P points xyz [P, 3] (normalised coordinates, fp32) to at most S of them.  A point with a non-finite
+ * coordinate is invalid and takes part in nothing.  For a valid point, per axis a:
+ *   q_a = clamp(floor(fl(x_a + 1) * 2^20), 0, 2^21 - 1)   (fp32 add, exact multiply, clamp in float, then integer)
+ *   level L = 0..21: cell k_a = q_a >> (21 - L), key = (k_x << 42) | (k_y << 21) | k_z,
+ *   e = sum_a (2 q_a + 1 - (2 k_a + 1) 2^(21 - L))^2 (exact int64: the squared distance to the cell centre, in units of
+ *   2^-21 / 2).
+ * n_L = the number of distinct occupied cells at level L (non-decreasing in L).  L* = the smallest L with n_L >= S, or 21.
+ * Each occupied cell at L* has one representative, the point of smallest (e, index).  When n_L* > S only the S
+ * representatives of smallest (h(key), key) are kept, h(key) = the splitmix64 finaliser of psam_mesh_sample_f32 applied to
+ * seed + (key + 1) * 0x9E3779B97F4A7C15 (mod 2^64); h is a bijection of the key, so the order is the order of h.
+ * Outputs: idx_out [S] int64 = the kept point indices in ascending order, then -1; stats (device int64 [4]) = (valid points,
+ * L*, n_L*, kept = min(S, n_L*)).
+ * Method: the level-21 keys; a binary search for L* over 0..21 (five steps, each counting the distinct cells of one level in
+ * an open-addressing hash set of 2^ceil(log2(2 P)) slots); the set of level L* with each cell's smallest e (atomicMin) and
+ * then its smallest index among the points with that e; the S-th smallest h by an 8-pass radix select; a flag per kept point
+ * and a stable compaction.  The result does not depend on the schedule.  34 launches and 10 memsets, no host
+ * synchronisation.  1 <= P <= 2^31 - 1, S >= 1.  workspace: psam_voxel_subsample_workspace_bytes(P) bytes, about
+ * 25 P + 20 * 2^ceil(log2(2 P)) (0.9 GB at P = 10^7), 16-byte aligned.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+size_t psam_voxel_subsample_workspace_bytes(int P);
+int psam_voxel_subsample_f32(const float* xyz, int P, int S, unsigned long long seed, long long* idx_out, long long* stats,
+                             void* workspace, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

@@ -18,11 +18,6 @@ constexpr int KNN_THREADS = 256;
 constexpr int KNN_MAX_CAP = 16384;     // candidate list capacity limit
 constexpr int KNN_MAX_SAMPLE = 16384;  // sample size limit (bounds the cost of phase A)
 
-__device__ __forceinline__ float sqdist3(float x, float y, float z, float cx, float cy, float cz) {
-    const float dx = x - cx, dy = y - cy, dz = z - cz;
-    return __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
-}
-
 // Block-wide sum of per-thread counts through one shared counter slot (one __syncthreads).
 __device__ __forceinline__ int block_count(int c, int* slot) {
     c = __reduce_add_sync(0xffffffffu, c);

@@ -94,32 +94,6 @@ __device__ __forceinline__ int pow2_exponent(unsigned bits) {
     return (31 - __clz((int)(bits & 0x7fffffu))) - 148;
 }
 
-// inclusive block scan of one uint64 per thread (kScan threads); returns the block total through `total`
-__device__ __forceinline__ unsigned long long block_scan_u64(unsigned long long x, unsigned long long* sw, unsigned long long& total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, off);
-        if (lane >= off) x += y;
-    }
-    if (lane == 31) sw[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        unsigned long long s = lane < kScan / 32 ? sw[lane] : 0ull;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-            const unsigned long long y = __shfl_up_sync(0xffffffffu, s, off);
-            if (lane >= off) s += y;
-        }
-        sw[lane] = s;  // inclusive warp totals
-    }
-    __syncthreads();
-    if (warp) x += sw[warp - 1];
-    total = sw[kScan / 32 - 1];
-    __syncthreads();  // sw is reused by the caller's next scan
-    return x;
-}
-
 __global__ void __launch_bounds__(kScan) mesh_scan_block_kernel(const float* __restrict__ a2, int F, const unsigned* __restrict__ maxbits,
                                                                 unsigned long long* __restrict__ cdf, unsigned long long* __restrict__ bsum) {
     psam::pdl_prologue();
@@ -130,24 +104,14 @@ __global__ void __launch_bounds__(kScan) mesh_scan_block_kernel(const float* __r
     // q = floor(A2 * 2^(32 - E)) < 2^32: the product of a float and a power of two is exact in fp64
     const unsigned long long q = f < F ? (unsigned long long)floor(__dmul_rn((double)a2[f], scale)) : 0ull;
     unsigned long long total;
-    const unsigned long long x = block_scan_u64(q, sw, total);
+    const unsigned long long x = psam::block_scan_u64<kScan>(q, sw, total);
     if (f < F) cdf[f] = x;
     if (threadIdx.x == 0) bsum[blockIdx.x] = total;
 }
 
 __global__ void __launch_bounds__(kScan) mesh_scan_sums_kernel(unsigned long long* __restrict__ bsum, int nb, long long* __restrict__ stats) {
     psam::pdl_prologue();
-    __shared__ unsigned long long sw[32];
-    unsigned long long carry = 0;
-    for (int base = 0; base < nb; base += kScan) {
-        const int i = base + threadIdx.x;
-        const unsigned long long v = i < nb ? bsum[i] : 0ull;
-        unsigned long long total;
-        const unsigned long long x = block_scan_u64(v, sw, total);
-        if (i < nb) bsum[i] = carry + x - v;  // exclusive
-        carry += total;
-    }
-    if (threadIdx.x == 0) stats[0] = (long long)carry;
+    psam::scan_block_sums<kScan>(bsum, nb, reinterpret_cast<unsigned long long*>(stats));  // the total weight goes to stats[0]
 }
 
 __global__ void __launch_bounds__(kScan) mesh_scan_add_kernel(unsigned long long* __restrict__ cdf, int F,

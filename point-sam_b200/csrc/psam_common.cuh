@@ -104,6 +104,58 @@ __device__ __forceinline__ float gelu_erf(float x) {
 
 __device__ __forceinline__ float silu(float x) { return x / (1.0f + __expf(-x)); }
 
+// Squared distance of the exact nearest-neighbour searches (psam_nn_distance_f32, psam_knn_f32, psam_nn_grid_f32):
+// dx = x - cx etc., fma(dz, dz, fma(dy, dy, dx * dx)), each step rounded once.
+__device__ __forceinline__ float sqdist3(float x, float y, float z, float cx, float cy, float cz) {
+    const float dx = x - cx, dy = y - cy, dz = z - cz;
+    return __fmaf_rn(dz, dz, __fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+}
+
+// Inclusive block scan of one uint64 per thread (NT threads, a multiple of 32, at most 1024); returns the block total
+// through `total`.  sw holds 32 words of shared memory.
+template <int NT>
+__device__ __forceinline__ unsigned long long block_scan_u64(unsigned long long x, unsigned long long* sw, unsigned long long& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xffffffffu, x, off);
+        if (lane >= off) x += y;
+    }
+    if (lane == 31) sw[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned long long s = lane < NT / 32 ? sw[lane] : 0ull;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xffffffffu, s, off);
+            if (lane >= off) s += y;
+        }
+        sw[lane] = s;  // inclusive warp totals
+    }
+    __syncthreads();
+    if (warp) x += sw[warp - 1];
+    total = sw[NT / 32 - 1];
+    __syncthreads();  // sw is reused by the caller's next scan
+    return x;
+}
+
+// One CTA of NT threads: exclusive scan in place of the nb block totals of a multi-block scan; the grand total goes to
+// *total when it is not NULL.
+template <int NT>
+__device__ __forceinline__ void scan_block_sums(unsigned long long* sums, int nb, unsigned long long* total) {
+    __shared__ unsigned long long sw[32];
+    unsigned long long carry = 0;
+    for (int base = 0; base < nb; base += NT) {
+        const int i = base + threadIdx.x;
+        const unsigned long long v = i < nb ? sums[i] : 0ull;
+        unsigned long long t;
+        const unsigned long long x = block_scan_u64<NT>(v, sw, t);
+        if (i < nb) sums[i] = carry + x - v;
+        carry += t;
+    }
+    if (threadIdx.x == 0 && total) *total = carry;
+}
+
 enum Act { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
 
 __device__ __forceinline__ float apply_act(float x, int act) {

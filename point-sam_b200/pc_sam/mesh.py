@@ -6,12 +6,12 @@ the mesh.  Here every step runs on the GPU:
 * ``sample_surface``  area-weighted surface samples (``psam_mesh_sample_f32``): faces are chosen in proportion to their
   area through an exact integer CDF, points are placed with the barycentric rule of the upstream browser demo, and the
   colour comes from vertex colours or from a texture (nearest texel).  The samples depend only on the mesh and the seed.
-* ``nearest_samples`` the nearest sample of every target point (``psam_nn_distance_f32``, exact, ties to the lower index).
+* ``nearest_samples`` the nearest sample of every target point (``psam_nn_grid_f32``: exact, ties to the lower index, bit
+  for bit the brute-force ``psam_nn_distance_f32``).
 * ``lift_masks``      bit-packed masks over the samples carried to the targets through their nearest sample (``psam_mask_lift``).
 * ``mask_labels``     one part label per point: the smallest mask containing it (``psam_mask_label_map``).
 
-The same lifting serves scans denser than the model's input: subsample, segment, then ``lift_masks`` with
-``nearest_samples(subsample, scan)``.
+The same lifting serves scans denser than the model's input: ``pc_sam.scan.ScanSegmenter`` subsamples, segments and lifts.
 
 ``MeshSegmenter`` ties these to a model (``PointCloudSAM`` or ``PointCloudSAMHier``, through its public API only): one
 sampling, encode and nearest-sample search per mesh, then prompted masks (``predict_masks``) or segment-everything
@@ -55,9 +55,7 @@ def sample_surface(vertices: torch.Tensor, faces: torch.Tensor, num_points: int,
 def nearest_samples(sample_xyz: torch.Tensor, target_xyz: torch.Tensor) -> torch.Tensor:
     """Index of the nearest sample of every target point (exact squared distance, ties to the lower index): int64 [M].
     A target with a NaN coordinate gets -1, which lift_masks reads as "in no mask"."""
-    s = sample_xyz.reshape(1, -1, 3).float().contiguous()
-    t = target_xyz.reshape(1, -1, 3).float().contiguous()
-    return ops.nn_index(t, s)[0]
+    return ops.nearest_grid(target_xyz, sample_xyz)[1]
 
 
 def lift_masks(bits: torch.Tensor, nearest: torch.Tensor, S: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -92,18 +90,88 @@ def _host(x, dtype) -> Optional[np.ndarray]:
     return np.asarray(x, dtype=dtype)
 
 
-class MeshSegmenter:
-    """Segment a triangle mesh with a Point-SAM model: the mesh is normalised (centroid at the origin, farthest vertex at
-    distance 1), num_points samples of its surface are encoded once, and masks over the samples are carried to every vertex
-    and face through their nearest sample (a face through its centre)."""
+class _SampleSegmenter:
+    """What MeshSegmenter and ScanSegmenter share: a model encoded once on S samples (self.xyz / self.rgb [1, S, 3]), and
+    named sets of target points, each carried by the index of its nearest sample (-1: no sample, so in no mask).
+    Subclasses set self.shift / self.scale (normalised = (x - shift) / scale) and self.targets = {name: nearest [M] int64}."""
 
-    def __init__(self, model, num_points: int = 32768, seed: int = 0):
+    def __init__(self, model, num_points: int, seed: int):
         if num_points < 1:
             raise ValueError(f"num_points must be >= 1, got {num_points}")
         self.model = model
         self.num_points = int(num_points)
         self.seed = int(seed)
-        self.xyz = self.rgb = self.face_index = None
+        self.xyz = self.rgb = None
+        self.targets: Dict[str, torch.Tensor] = {}
+
+    def _require(self):
+        if self.xyz is None:
+            raise RuntimeError(f"call {self._setter}() first")
+
+    def normalize(self, points) -> np.ndarray:
+        """Points in input coordinates -> the normalised coordinates of the samples (float64 on the host, then float32)."""
+        self._require()
+        return ((_host(points, np.float64) - self.shift) / self.scale).astype(np.float32)
+
+    @staticmethod
+    def _gather(x: torch.Tensor, near: torch.Tensor, dim: int, fill):
+        """x gathered along dim through near; entries with near < 0 take `fill`."""
+        got = x.index_select(dim, near.clamp(min=0))
+        miss = (near < 0).view([-1 if d == dim else 1 for d in range(x.dim())])
+        return got.masked_fill(miss, fill)
+
+    def predict_masks(self, prompt_points, prompt_labels, prompt_mask=None, multimask_output: bool = True) -> Dict[str, torch.Tensor]:
+        self._require()
+        dev = self.xyz.device
+        pts = torch.from_numpy(self.normalize(np.asarray(_host(prompt_points, np.float64)).reshape(-1, 3))).to(dev)[None]
+        labels = torch.from_numpy(_host(prompt_labels, np.int64).reshape(1, -1)).to(dev)
+        logits, scores, _ = self.model.predict_masks(pts, labels, prompt_mask, multimask_output)
+        logits, scores = logits[0], scores[0]
+        out = dict(logits=logits, scores=scores)
+        for name, near in self.targets.items():
+            out[f"{name}_logits"] = self._gather(logits, near, 1, float("-inf"))
+        return out
+
+    def lift_packed(self, out: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        self._require()
+        S = self.xyz.shape[1]
+        bits, area = out["bits"], out["area"]
+        res = dict(out)
+        for name, near in self.targets.items():
+            res[f"{name}_bits"], res[f"{name}_area"] = lift_masks(bits, near, S)
+        labels = mask_labels(bits, area, S)
+        res["sample_labels"] = labels
+        for name, near in self.targets.items():
+            res[f"{name}_labels"] = self._gather(labels, near, 0, -1)
+        res.update(self._extras())
+        return res
+
+    def _extras(self) -> Dict:
+        return dict(shift=self.shift, scale=self.scale)
+
+    def generate_packed(self, generator, **kwargs) -> Dict[str, torch.Tensor]:
+        self._require()
+        return self.lift_packed(generator.generate_packed(self.xyz, self.rgb, **kwargs))
+
+
+class MeshSegmenter(_SampleSegmenter):
+    """Segment a triangle mesh with a Point-SAM model: the mesh is normalised (centroid at the origin, farthest vertex at
+    distance 1), num_points samples of its surface are encoded once, and masks over the samples are carried to every vertex
+    and face through their nearest sample (a face through its centre)."""
+
+    _setter = "set_mesh"
+
+    def __init__(self, model, num_points: int = 32768, seed: int = 0):
+        super().__init__(model, num_points, seed)
+        self.face_index = None
+
+    @property
+    def vertex_nearest(self) -> torch.Tensor:
+        return self.targets["vertex"]
+
+    @property
+    def face_nearest(self) -> torch.Tensor:
+        return self.targets["face"]
 
     def set_mesh(self, vertices, faces, vertex_colors=None, uv=None, texture=None):
         """vertices [V, 3], faces [F, 3] and the optional colour sources of sample_surface (numpy arrays or tensors).  Samples
@@ -129,43 +197,18 @@ class MeshSegmenter:
         self.xyz, self.rgb, self.face_index = xyz[None], rgb[None], face
         self.model.set_pointcloud(self.xyz, self.rgb)
         self.face_centers = ops.mesh_face_centers(vn, f)
-        self.vertex_nearest = nearest_samples(xyz, vn)
-        self.face_nearest = nearest_samples(xyz, self.face_centers)
-
-    def _require_mesh(self):
-        if self.xyz is None:
-            raise RuntimeError("call set_mesh() first")
-
-    def normalize(self, points) -> np.ndarray:
-        """Points in mesh coordinates -> the normalised coordinates of the samples (float64 on the host, then float32)."""
-        self._require_mesh()
-        return ((_host(points, np.float64) - self.shift) / self.scale).astype(np.float32)
+        self.targets = dict(vertex=nearest_samples(xyz, vn), face=nearest_samples(xyz, self.face_centers))
 
     def predict_masks(self, prompt_points, prompt_labels, prompt_mask=None, multimask_output: bool = True) -> Dict[str, torch.Tensor]:
         """Prompted masks: prompt_points [P, 3] in mesh coordinates, prompt_labels [P] (1 foreground, 0 background),
         prompt_mask [1, S] logits over the samples or None.  Returns logits [C, S] and scores [C] over the samples, and
         vertex_logits [C, V] / face_logits [C, F], each element taking its nearest sample's logits."""
-        self._require_mesh()
-        dev = self.xyz.device
-        pts = torch.from_numpy(self.normalize(np.asarray(_host(prompt_points, np.float64)).reshape(-1, 3))).to(dev)[None]
-        labels = torch.from_numpy(_host(prompt_labels, np.int64).reshape(1, -1)).to(dev)
-        logits, scores, _ = self.model.predict_masks(pts, labels, prompt_mask, multimask_output)
-        logits, scores = logits[0], scores[0]
-        return dict(logits=logits, scores=scores, vertex_logits=logits.index_select(1, self.vertex_nearest),
-                    face_logits=logits.index_select(1, self.face_nearest))
+        return super().predict_masks(prompt_points, prompt_labels, prompt_mask, multimask_output)
 
     def lift_packed(self, out: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
         """generate_packed's output over the samples, with the masks and labels of the vertices and faces added (see
         generate_packed).  Nothing here waits for the device."""
-        self._require_mesh()
-        S = self.xyz.shape[1]
-        bits, area = out["bits"], out["area"]
-        vbits, varea = lift_masks(bits, self.vertex_nearest, S)
-        fbits, farea = lift_masks(bits, self.face_nearest, S)
-        labels = mask_labels(bits, area, S)
-        return dict(out, vertex_bits=vbits, vertex_area=varea, face_bits=fbits, face_area=farea, sample_labels=labels,
-                    vertex_labels=labels.index_select(0, self.vertex_nearest),
-                    face_labels=labels.index_select(0, self.face_nearest), shift=self.shift, scale=self.scale)
+        return super().lift_packed(out)
 
     def generate_packed(self, generator, **kwargs) -> Dict[str, torch.Tensor]:
         """PointCloudMaskGenerator.generate_packed on the samples (keywords such as min_mask_region_area and the crop_*
@@ -177,5 +220,4 @@ class MeshSegmenter:
           vertex_labels [V] / face_labels [F] int32: the label of each element's nearest sample,
           shift [3] and scale: normalised = (mesh - shift) / scale.
         The lifting and the labels add no host synchronisation to the generator's own."""
-        self._require_mesh()
-        return self.lift_packed(generator.generate_packed(self.xyz, self.rgb, **kwargs))
+        return super().generate_packed(generator, **kwargs)

@@ -69,6 +69,7 @@ EXPORTS = [
     "psam_crop_total", "psam_crop_layout_f32", "psam_crop_gather_workspace_bytes", "psam_crop_gather_f32", "psam_crop_edge_filter",
     "psam_crop_uncrop",
     "psam_mesh_sample_workspace_bytes", "psam_mesh_sample_f32", "psam_mesh_face_centers_f32", "psam_mask_lift", "psam_mask_label_map",
+    "psam_nn_grid_workspace_bytes", "psam_nn_grid_f32", "psam_voxel_subsample_workspace_bytes", "psam_voxel_subsample_f32",
     "psam_version",
 ]
 
@@ -99,6 +100,10 @@ def lib():
         L.psam_crop_gather_workspace_bytes.argtypes = [i]
         L.psam_mesh_sample_workspace_bytes.restype = c_size_t
         L.psam_mesh_sample_workspace_bytes.argtypes = [i]
+        L.psam_nn_grid_workspace_bytes.restype = c_size_t
+        L.psam_nn_grid_workspace_bytes.argtypes = [i]
+        L.psam_voxel_subsample_workspace_bytes.restype = c_size_t
+        L.psam_voxel_subsample_workspace_bytes.argtypes = [i]
         sig = {
             "psam_fps_f32": [p, i, i, i, p, p, p, p],
             "psam_knn_f32": [p, p, i, i, i, i, p, p, p],
@@ -143,6 +148,8 @@ def lib():
             "psam_mesh_face_centers_f32": [p, i, p, i, p, p],
             "psam_mask_lift": [p, i, i, i, p, i, i, p, p, p],
             "psam_mask_label_map": [p, i, i, p, i, p, p],
+            "psam_nn_grid_f32": [p, i, p, i, p, p, p, p],
+            "psam_voxel_subsample_f32": [p, i, i, ctypes.c_uint64, p, p, p, p],
         }
         for name, args in sig.items():
             fn = getattr(L, name)

@@ -597,3 +597,34 @@ def mask_label_map(bits: torch.Tensor, priority: torch.Tensor, N: int) -> torch.
     nv.check(nv.lib().psam_mask_label_map(nv.ptr(b) if K else None, K, W, nv.ptr(pr) if K else None, int(N), nv.ptr(labels),
                                           nv.stream()), "mask_label_map")
     return labels
+
+
+# ------------------------------------------------------------------------------------------------
+# dense scans
+# ------------------------------------------------------------------------------------------------
+def nearest_grid(query: torch.Tensor, key: torch.Tensor):
+    """Nearest key of every query point on a uniform grid (psam_nn_grid_f32): query [n1, 3], key [n2, 3] (any leading shape,
+    fp32).  Returns (dist [n1] fp32, idx [n1] int64), bit for bit those of psam_nn_distance_f32: exact squared distance, ties
+    to the lower key index, (3.4e38, -1) for a query with no finite distance.  Nothing waits for the device."""
+    q = query.reshape(-1, 3).float().contiguous()
+    k = key.reshape(-1, 3).float().contiguous()
+    n1, n2, dev = q.shape[0], k.shape[0], q.device
+    dist = torch.empty(n1, dtype=torch.float32, device=dev)
+    idx = torch.empty(n1, dtype=torch.int64, device=dev)
+    ws = torch.empty(nv.lib().psam_nn_grid_workspace_bytes(n2), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_nn_grid_f32(nv.ptr(q), n1, nv.ptr(k), n2, nv.ptr(dist), nv.ptr(idx), nv.ptr(ws), nv.stream()), "nn_grid")
+    return dist, idx
+
+
+def voxel_subsample(xyz: torch.Tensor, S: int, seed: int = 0):
+    """At most S points of xyz [P, 3] (normalised fp32), one per occupied voxel of the coarsest level with at least S voxels
+    (psam_voxel_subsample_f32).  Returns (idx [S] int64: the kept indices ascending, then -1; stats [4] int64 = (valid
+    points, level, occupied voxels, kept)), both on the device; nothing waits for it."""
+    x = xyz.reshape(-1, 3).float().contiguous()
+    P, dev = x.shape[0], x.device
+    idx = torch.empty(int(S), dtype=torch.int64, device=dev)
+    stats = torch.empty(4, dtype=torch.int64, device=dev)
+    ws = torch.empty(nv.lib().psam_voxel_subsample_workspace_bytes(P), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_voxel_subsample_f32(nv.ptr(x), P, int(S), int(seed) & (2 ** 64 - 1), nv.ptr(idx), nv.ptr(stats), nv.ptr(ws),
+                                               nv.stream()), "voxel_subsample")
+    return idx, stats

@@ -106,3 +106,36 @@ def make_mesh(num_faces: int, seed: int = 0):
         cs.append(np.tile(rng.uniform(0, 1, 3), (len(v), 1)))
         base += len(v)
     return np.concatenate(vs), np.concatenate(fs), np.concatenate(cs).astype(np.float32)
+
+
+def make_scan(P: int, seed: int = 0):
+    """A LiDAR-like scan of P points over the make_mesh scene (about 20k faces): (xyz [P, 3] float32, rgb [P, 3] float32 in
+    0..1).  Points are surface samples kept with probability falling off as 1 / (1 + (r / 2)^2) with the distance r from a
+    sensor at (0, 0, 3), so the density falls with range; a few rows are NaN and a few are far outliers (up to 50 times the
+    scene's size)."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+    v, f, col = make_mesh(20000, seed)
+    a, b, c = v[f[:, 0]].astype(np.float64), v[f[:, 1]].astype(np.float64), v[f[:, 2]].astype(np.float64)
+    area = 0.5 * np.linalg.norm(np.cross(b - a, c - a), axis=1)
+    cdf = np.cumsum(area) / area.sum()
+    sensor = np.array([0.0, 0.0, 3.0])
+    out_xyz, out_rgb, n = [], [], 0
+    while n < P:
+        m = max(2 * (P - n), 1024)
+        face = np.minimum(np.searchsorted(cdf, rng.random(m)), len(f) - 1)
+        r1, r2 = np.sqrt(rng.random(m))[:, None], rng.random(m)[:, None]
+        p = (1 - r1) * a[face] + r1 * (1 - r2) * b[face] + r1 * r2 * c[face]
+        r = np.linalg.norm(p - sensor, axis=1)
+        keep = rng.random(m) < 1.0 / (1.0 + (r / 2.0) ** 2)
+        out_xyz.append(p[keep])
+        out_rgb.append(col[f[face[keep], 0]])
+        n += int(keep.sum())
+    xyz = np.concatenate(out_xyz)[:P].astype(np.float32)
+    rgb = np.concatenate(out_rgb)[:P].astype(np.float32)
+    k = max(1, P // 10000)
+    rows = rng.choice(P, min(P, 2 * k), replace=False)
+    xyz[rows[:k], rng.integers(0, 3, len(rows[:k]))] = np.nan
+    xyz[rows[k:]] = rng.uniform(-1, 1, (len(rows[k:]), 3)).astype(np.float32) * np.float32(200)
+    return xyz, rgb

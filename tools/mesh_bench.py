@@ -4,7 +4,7 @@ S = 32768 surface samples, the c2 model (eva02_large_patch14_448, 512 x 64 group
 
 Prints one JSON line: device name and power limit (read in the same run), and per mesh the ms of each stage by CUDA events
 (median of --steps after --warmup, all in the same run): surface sampling (including its one statistics read), face centres,
-nearest samples of the vertices and of the faces (brute force, M x S distances), lifting to vertices and faces plus the label
+nearest samples of the vertices and of the faces (the exact grid search psam_nn_grid_f32), lifting to vertices and faces plus the label
 maps, and generate_packed on the sampled cloud; then the kernel times of each stage from a separate torch.profiler run.
 usage: python tools/mesh_bench.py [--steps 5] [--warmup 1] [--faces 200000,2000000]"""
 import argparse
