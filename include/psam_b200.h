@@ -68,8 +68,9 @@ int psam_voronoi_features_f32(const float* xyz, const float* centers, const long
                               cudaStream_t stream);
 
 /* y[b, nn_idx[b,n], :] = max over the points of a Voronoi cell of x[b,n,:]; cells without a point are 0.
- * Replaces y.scatter_reduce_(1, nn_idx, x, "amax", include_self=False) on a zero tensor (pc_encoder.py:189-193).
- * x [B,N,D], y [B,G,D], D % 4 == 0. */
+ * Replaces y.scatter_reduce_(1, nn_idx, x, "amax", include_self=False) on a zero tensor (pc_encoder.py:189-193), bit for
+ * bit: the maximum is exact, and -0.0 orders below +0.0 and above every negative value (a cell holding -0.0 and negative
+ * values gives -0.0).  NaN inputs are outside this contract.  x [B,N,D], y [B,G,D], D % 4 == 0. */
 int psam_scatter_amax_f32(const float* x, const long long* nn_idx, int B, int N, int G, int D, float* y,
                           cudaStream_t stream);
 
@@ -127,7 +128,8 @@ typedef struct {
     int tile_hint;          /* 0: tile width for lowest latency; 1: for lowest SM-time (several clouds in flight); 32..256: explicit
                                (a multiple of 32, rounded up to the tile widths the kernel has: 64, 128, 256) */
     float* gmax;            /* optional fused max-pool: gmax[(row / group_rows) * ld_gmax + col] = max over the group rows
-                               (atomic; caller pre-fills with -inf; group_rows multiple of 32); replaces torch.max(x, dim=-2) */
+                               (atomic; caller pre-fills with -inf; group_rows multiple of 32); replaces torch.max(x, dim=-2).
+                               -0.0 orders below +0.0 and above every negative value; NaN values are outside this contract */
     long long ld_gmax;
     int group_rows;
     const float* rd_w;      /* optional fused row-dot (replaces masks = hyper_in @ upscaled^T, mask_decoder.py:176):        */
@@ -231,7 +233,7 @@ int psam_swiglu_ln(const float* gx, long long ld, long long x_off, int rows, int
                    cudaStream_t stream);
 
 /* First layer of the mini-PointNet / positional MLP: y = act(LN?(x[rows,Cin] * W[Cout,Cin]^T + b)),
- * Cin <= 8, Cout multiple of 32 and <= 512; split-bf16 output.  Replaces conv1[0..2] of PatchEncoder
+ * Cin <= 16, Cout in {32, 64, 128, 256, 512} (another multiple of 32 -> PSAM_ERR_UNSUPPORTED); split-bf16 output.  Replaces conv1[0..2] of PatchEncoder
  * (common.py:486-489) and pos_embed[0..1] (pc_encoder.py:102-104). */
 int psam_small_in_linear(const float* x, int rows, int Cin, const float* W, const float* b, const float* gamma,
                          const float* beta, float eps, int use_ln, int act, int Cout, void* y_hi, long long y_plane,
@@ -260,12 +262,20 @@ int psam_posenc_f32(const float* coords, long long rows, const float* gauss, int
 
 /* Multi-head softmax attention for short sequences (fp32, one warp per query):
  * O[z,i,h,:] = softmax(Q[z,i,h,:] . K[z,:,h,:]^T / sqrt(dh)) V[z,:,h,:].  Replaces
- * Attention.forward core (transformer.py:214-233). */
+ * Attention.forward core (transformer.py:214-233).  dh in {8, 16, 32, 64} and Lk <= 12798 - 2*dh (the scores of four
+ * queries stay in shared memory); otherwise PSAM_ERR_UNSUPPORTED. */
 int psam_attention_f32(const float* q, const float* k, const float* v, float* o, int Z, int Lq, int Lk, int H, int dh,
                        long long ldq, long long ldk, long long ldv, long long ldo, cudaStream_t stream);
 
-/* Mask-decoder glue (mask_decoder.py:126-139): tokens[z] = cat(iou_token, mask_tokens, sparse[z]);
- * src[z,g,:] = pc_emb[z/rep,g,:] + dense[(z % dense_mod)...]; see engine for exact broadcast rules. */
+/* Mask-decoder glue (mask_decoder.py:126-139).  With T = 1 + n_mask_tokens + P, for z < Z, g < G, d < D:
+ *   tokens[(z*T + t)*D + d] = iou_token[d]                                 (t = 0)
+ *                           = mask_tokens[(t-1)*D + d]                     (1 <= t <= n_mask_tokens)
+ *                           = sparse[(z*P + t-1-n_mask_tokens)*D + d]      (t > n_mask_tokens)
+ *   src[(z*G + g)*D + d]    = pc_emb[((z/rep)*G + g)*D + d] + dense[z*dense_z + g*dense_g + d]   (one fp32 add)
+ * i.e. tokens = cat(iou_token, mask_tokens, sparse[z]) and src = repeat_interleave(pc_emb, rep) + dense.  The engine
+ * passes dense in three forms: the no-mask embedding [D] broadcast to every (z, g) (dense_z = dense_g = 0), one map per
+ * prompt [Z,G,D] (dense_z = G*D, dense_g = D), and one map for all prompts [1,G,D] (dense_z = 0, dense_g = D).
+ * sparse may be NULL when P == 0. */
 int psam_decoder_prepare(const float* iou_token, const float* mask_tokens, int n_mask_tokens, const float* sparse,
                          int P, const float* pc_emb, const float* dense, long long dense_z, long long dense_g, int Z,
                          int rep, int G, int D, float* tokens, float* src, cudaStream_t stream);

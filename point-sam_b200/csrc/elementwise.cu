@@ -348,8 +348,12 @@ __global__ void fill_f32_kernel(float* __restrict__ y, long long n, float v) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) y[i] = v;
 }
 
+// Float max through integer atomics, branching on the sign bit: non-negative patterns order like signed ints, negative
+// ones in reverse like unsigned ints, and -0.0 (0x80000000) takes the unsigned side, so it beats every negative value
+// and loses to +0.0.  (A `v >= 0.f` branch sent -0.0 to the signed side, where it is INT_MIN and never wins.)  NaN inputs
+// are not ordered by this.
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-    if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
@@ -463,7 +467,7 @@ __global__ void posenc_kernel(const float* __restrict__ coords, long long rows, 
     }
 }
 
-// one warp per (z, head, query); scores kept in shared memory (Lk <= 4096).  Both phases split the KEYS across
+// one warp per (z, head, query); scores kept in shared memory (Lk <= 12798 - 2*dh, the host's 200 KB check).  Both phases split the KEYS across
 // lanes (the value phase accumulates dh partial sums per lane and reduces them with shuffles), so long
 // key sequences (tokens -> 512 patches) do not serialise on one lane.
 template <int DH, int WPI>  // WPI warps cooperate on one (z, head, query) item, each taking a slice of the keys

@@ -165,8 +165,10 @@ __device__ __forceinline__ void epi_rows_split(const float* __restrict__ stg, in
 }
 
 
+// Float max through integer atomics, branching on the sign bit so that -0.0 takes the unsigned-min side (see
+// atomic_max_float in elementwise.cu); NaN inputs are not ordered by this.
 __device__ __forceinline__ void atomic_max_f32(float* addr, float v) {
-    if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
