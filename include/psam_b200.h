@@ -117,13 +117,18 @@ typedef struct {
 typedef struct {
     float* out_f32;         /* optional fp32 output [.., M, ldo] */
     long long ldo, out_b1, out_b2;
-    void* out_hi;           /* optional split-bf16 output (hi plane; lo at +out_plane elements) */
+    void* out_hi;           /* optional split-bf16 output (hi plane; lo at +out_plane elements).  Any bf16-aligned address:
+                             * the vectorised epilogue runs when out_hi is 8-byte aligned and ldo_s, out_plane, outs_b1,
+                             * outs_b2 are multiples of 4; otherwise the scalar one stores column pairs as 32-bit words
+                             * only when out_hi is 4-byte aligned and those strides are even, and single bf16 otherwise */
     long long out_plane, ldo_s, outs_b1, outs_b2;
     const float* bias;      /* [N] or NULL */
     const float* resid;     /* fp32, geometry of out_f32 (may alias it) or NULL */
     float alpha;            /* accumulator scale (1.0f for a plain linear) */
     int act;                /* PSAM_ACT_* applied after bias/residual */
-    int accumulate;         /* 1: out_f32 += alpha*acc (+bias) with red.add; required when split_k>1 */
+    int accumulate;         /* 1: out_f32 += alpha*acc (+bias) with red.add; required when split_k>1.  Needs out_f32, and
+                             * out_hi == NULL, act == 0, resid NULL or == out_f32 (out_f32 is its own residual);
+                             * PSAM_ERR_ARG otherwise */
     int swiglu;             /* 1: W rows interleaved (gate_i, value_i); out_f32[:, i] = silu(gate_i)*value_i (fp32 out only) */
     int tile_hint;          /* 0: tile width for lowest latency; 1: for lowest SM-time (several clouds in flight); 32..256: explicit
                                (a multiple of 32, rounded up to the tile widths the kernel has: 64, 128, 256) */
@@ -141,10 +146,10 @@ typedef struct {
                              * accumulate) the final values after bias / residual / activation (norm1 / norm2 / fc_norm) */
     const float* ln_stats;  /* LayerNorm folded into this GEMM: A = the un-normalised rows, W pre-multiplied by gamma,
                              * ln_c[n] = sum_k gamma_k W[n,k], bias[n] = sum_k beta_k W[n,k] + b[n];
-                             * out = act(rstd_row * (acc - mean_row * ln_c[n]) + bias[n] (+ resid)) with mean / rstd from
-                             * ln_stats[row] = (sum, sum sq) over ln_h columns.  Works with every output form of the
-                             * vectorised epilogue (fp32, split-bf16, SwiGLU pairs) and with accumulate / split_k (each
-                             * split scales its partial sum). */
+                             * out = act(alpha * rstd_row * (acc - mean_row * ln_c[n]) + bias[n] (+ resid)) with mean / rstd
+                             * from ln_stats[row] = (sum, sum sq) over ln_h columns; bias may be NULL.  Works with every
+                             * output form of the vectorised epilogue (fp32, split-bf16, SwiGLU pairs) and with accumulate /
+                             * split_k (each split scales its partial sum; split 0 adds the mean term and the bias). */
     const float* ln_c;
     int ln_h;
     float ln_eps;
@@ -172,7 +177,8 @@ int psam_gemm_rowln_bf16x3(const psam_operand* a, const psam_operand* w, const f
  * q/k/v are split-bf16 operand views [L rows x dh] with nb1 = heads, nb2 = clouds (typically three column windows of
  * the fused qkv activation).  dh == 64 or 88 (EVA-giant; the 88-wide head is handled as 64 + 24 columns, zero padded by
  * TMA), any L >= 1 (PSAM_ERR_UNSUPPORTED otherwise - the caller then uses
- * psam_gemm_bf16x3 + psam_softmax_split).  Key blocks are streamed once: S_j = Q K_j^T stays in registers, the running row
+ * psam_gemm_bf16x3 + psam_softmax_split).  k and v must have q's rows, k, nb1 and nb2, and scale must be finite and > 0
+ * (PSAM_ERR_ARG otherwise).  Key blocks are streamed once: S_j = Q K_j^T stays in registers, the running row
  * maximum rescales O and the row sum when it grows, and P_j (split-bf16, in registers) is the A operand of the PV wgmma.
  * Replaces F.scaled_dot_product_attention in timm EvaAttention (blocks called at pc_encoder.py:138-139). */
 int psam_attention_bf16x3(const psam_operand* q, const psam_operand* k, const psam_operand* v, void* out_hi,

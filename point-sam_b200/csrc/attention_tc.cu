@@ -276,6 +276,11 @@ static int attention_setup(const psam_operand* q, const psam_operand* k, const p
     const int H = q->nb1 > 0 ? q->nb1 : 1, B = q->nb2 > 0 ? q->nb2 : 1;
     if ((dh != 64 && dh != 88) || L <= 0) return PSAM_ERR_UNSUPPORTED;
     if (k->rows != L || v->rows != L || k->k != dh || v->k != dh) return PSAM_ERR_ARG;
+    // K and V cover the same heads and clouds as Q (TMA would fill the missing ones with zeros)
+    for (const psam_operand* x : {k, v})
+        if ((x->nb1 > 0 ? x->nb1 : 1) != H || (x->nb2 > 0 ? x->nb2 : 1) != B) return PSAM_ERR_ARG;
+    // the kernels subtract the maximum of the raw scores, which is the maximum of the scaled ones only for scale > 0
+    if (!(scale > 0.f) || !isfinite(scale)) return PSAM_ERR_ARG;
     if ((ldo | out_plane | out_head_stride | out_cloud_stride) & 7) return PSAM_ERR_ARG;
     int rc = make_operand_map_ext(mq, q, ATT_BQ, 2);
     if (rc) return rc;

@@ -61,7 +61,7 @@ struct GemmEpilogue {
     int rd_rows, rd_c;
     float* stats_out;        // SwiGLU + split output: stats_out[row] += (sum, sum of squares) of the fp32 products of the row
     const float* ln_stats;   // LayerNorm folded into THIS GEMM: A holds the un-normalised rows, W is pre-scaled by gamma;
-    const float* ln_c;       //   out = rstd * (acc - mean * ln_c[n]) + bias[n]  (bias = W beta + b), stats = (sum, sum sq) per row
+    const float* ln_c;       //   out = alpha rstd (acc - mean ln_c[n]) + bias[n]  (bias = W beta + b), stats = (sum, sum sq) per row
     float ln_inv_h, ln_eps;
     int vec4;  // host-verified: every output / bias / residual row is 16-byte (split planes: 8-byte) addressable in 4-column steps
 };
@@ -182,7 +182,7 @@ __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast
 
 template <int ACT, bool RES, int MODE>
 __device__ __forceinline__ void epi_chunk_v4(const float* __restrict__ stg, int pitch, int lane, int row0, int M, int col0,
-                                             const GemmEpilogue& ep, bool add_bias, float* out, const float* res,
+                                             const GemmEpilogue& ep, bool add_bias, bool lead, float* out, const float* res,
                                              __nv_bfloat16* ohi) {
     const int cg = lane & 7, rsub = lane >> 3;
     const int col = col0 + cg * 4;
@@ -203,7 +203,8 @@ __device__ __forceinline__ void epi_chunk_v4(const float* __restrict__ stg, int 
             const float2 st = ok ? *reinterpret_cast<const float2*>(ep.ln_stats + 2 * (long long)row) : make_float2(0.f, 1.f);
             const float mean = st.x * ep.ln_inv_h;
             const float rstd = rsqrtf(fmaxf(fmaf(-mean, mean, st.y * ep.ln_inv_h), 0.f) + ep.ln_eps);
-            const float ra = rstd * alpha, mr = add_bias ? -mean * rstd : 0.f;
+            // alpha rstd (acc - mean c[n]) + bias'[n]: the mean term belongs to split 0 alone, whether or not there is a bias
+            const float ra = rstd * alpha, mr = lead ? -mean * ra : 0.f;
             x.x = fmaf(x.x, ra, fmaf(mr, c4.x, b4.x)), x.y = fmaf(x.y, ra, fmaf(mr, c4.y, b4.y));
             x.z = fmaf(x.z, ra, fmaf(mr, c4.z, b4.z)), x.w = fmaf(x.w, ra, fmaf(mr, c4.w, b4.w));
         } else {
@@ -291,9 +292,9 @@ __device__ __forceinline__ void epi_chunk_v4(const float* __restrict__ stg, int 
 
 template <int ACT>
 __device__ __forceinline__ void epi_chunk_v4_dispatch(const float* stg, int pitch, int lane, int row0, int M, int col0,
-                                                      const GemmEpilogue& ep, bool add_bias, float* out, const float* res,
+                                                      const GemmEpilogue& ep, bool add_bias, bool lead, float* out, const float* res,
                                                       __nv_bfloat16* ohi) {
-#define PSAM_V4(R, MODE) epi_chunk_v4<ACT, R, MODE>(stg, pitch, lane, row0, M, col0, ep, add_bias, out, res, ohi)
+#define PSAM_V4(R, MODE) epi_chunk_v4<ACT, R, MODE>(stg, pitch, lane, row0, M, col0, ep, add_bias, lead, out, res, ohi)
     if (ep.swiglu && ohi) PSAM_V4(false, EPI_SWIGLU_SPLIT);
     else if (ep.swiglu) PSAM_V4(false, EPI_SWIGLU);
     else if (ep.accumulate) PSAM_V4(false, EPI_ACC);
@@ -317,7 +318,8 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
         float* out = ep.out_f32 ? ep.out_f32 + obase : nullptr;
         const float* res = (ep.resid && !ep.accumulate) ? ep.resid + obase : nullptr;
         __nv_bfloat16* ohi = ep.out_hi ? ep.out_hi + (long long)b1 * ep.outs_b1 + (long long)b2 * ep.outs_b2 : nullptr;
-        const bool add_bias = ep.bias && split == 0;
+        const bool lead = split == 0;  // the split that adds the bias and the folded LayerNorm's mean term
+        const bool add_bias = ep.bias && lead;
         const int nchunks = BN / 32;
 #pragma unroll 1
         for (int c = ehalf; c < nchunks; c += 2) {
@@ -327,7 +329,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
             if (ep.rd_out) {
                 // fused "masks = hyper_in @ upscaled^T" (mask_decoder.py:176): thread = row, the activated row chunk is
                 // dotted with the rd_c hyper vectors and accumulated with one atomic per (row, c); the 32768 x 256
-                // upscaled embedding is never written
+                // upscaled embedding is never written.  Warps wholly past row M have nothing to add, and their batch
+                // index zz would read rd_w one batch past its end.
+                if (row0 >= shape.M) break;
                 const int row = row0 + lane;
                 const int zz = row0 / ep.rd_rows;
                 const float* wz = ep.rd_w + (long long)zz * ep.rd_c * shape.N;
@@ -354,9 +358,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
             }
             if (ep.vec4 && col0 + 32 <= shape.N) {
                 if (ep.swiglu || ep.accumulate || ep.act == ACT_NONE)
-                    epi_chunk_v4_dispatch<ACT_NONE>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
-                else if (ep.act == ACT_GELU) epi_chunk_v4_dispatch<ACT_GELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
-                else epi_chunk_v4_dispatch<ACT_RELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, out, res, ohi);
+                    epi_chunk_v4_dispatch<ACT_NONE>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, lead, out, res, ohi);
+                else if (ep.act == ACT_GELU) epi_chunk_v4_dispatch<ACT_GELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, lead, out, res, ohi);
+                else epi_chunk_v4_dispatch<ACT_RELU>(stg, pitch, lane, row0, shape.M, col0, ep, add_bias, lead, out, res, ohi);
                 continue;
             }
             const int col = col0 + lane;
@@ -389,7 +393,9 @@ __device__ __forceinline__ void gemm_epilogue(const GemmShape& shape, const Gemm
 #undef PSAM_EPI_F32
             } else {
                 const float* bias = add_bias ? ep.bias : nullptr;
-                const bool va = ((ep.ldo_s | ep.out_plane | ep.outs_b1 | ep.outs_b2) & 1) == 0;
+                // 32-bit stores of column pairs only where every pair is 4-byte aligned: even strides and out_hi itself
+                const bool va = ((ep.ldo_s | ep.out_plane | ep.outs_b1 | ep.outs_b2) & 1) == 0 &&
+                                (reinterpret_cast<uintptr_t>(ep.out_hi) & 3) == 0;
 #define PSAM_EPI_SP(A, R, F) epi_rows_split<A, R, F>(stg, pitch, lane, row0, shape.M, shape.N, col0, ep.alpha, bias, out, res, ep.ldo, ohi, ep.out_plane, ep.ldo_s, va)
 #define PSAM_EPI_SP_ACT(R, F)                                   \
     if (ep.act == ACT_NONE) PSAM_EPI_SP(ACT_NONE, R, F);        \
@@ -795,7 +801,10 @@ extern "C" int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, co
     if (a->k != w->k || a->k <= 0 || a->rows <= 0 || w->rows <= 0) return PSAM_ERR_ARG;
     if (passes != 1 && passes != 3) return PSAM_ERR_ARG;
     if (split_k < 1) split_k = 1;
-    if (split_k > 1 && !(o->accumulate && o->out_f32 && !o->out_hi && o->act == 0)) return PSAM_ERR_ARG;
+    // accumulate adds the pre-activation result into out_f32 (which is then its own residual): no split output, no
+    // activation, no other residual - neither epilogue has a form that would honour them
+    if (o->accumulate && !(o->out_f32 && !o->out_hi && o->act == 0 && (!o->resid || o->resid == o->out_f32))) return PSAM_ERR_ARG;
+    if (split_k > 1 && !o->accumulate) return PSAM_ERR_ARG;
     if (!o->out_f32 && !o->out_hi && !o->gmax && !o->rd_out) return PSAM_ERR_ARG;
     GemmShape sh;
     sh.M = a->rows, sh.N = w->rows, sh.K = a->k;
@@ -819,7 +828,7 @@ extern "C" int psam_gemm_bf16x3(const psam_operand* a, const psam_operand* w, co
         const bool off = (variant & GV_SCALAR_EPI) != 0;
         bool ok = !off && !ep.rd_out && (!ep.bias || a16(ep.bias));
         if (ep.out_f32) ok = ok && a16(ep.out_f32) && ((ep.ldo | ep.out_b1 | ep.out_b2) & 3) == 0;
-        if (ep.resid) ok = ok && a16(ep.resid);
+        if (ep.resid) ok = ok && a16(ep.resid) && ((ep.ldo | ep.out_b1 | ep.out_b2) & 3) == 0;  // also without out_f32
         if (ep.out_hi) ok = ok && a8(ep.out_hi) && ((ep.ldo_s | ep.out_plane | ep.outs_b1 | ep.outs_b2) & 3) == 0;
         if (ep.gmax) ok = ok && ep.group_rows % 32 == 0;
         ep.vec4 = ok ? 1 : 0;
