@@ -11,6 +11,11 @@
  * work is enqueued on `stream` and nothing synchronises; return 0 on success, a negative PSAM_ERR_*
  * for bad arguments, a positive cudaError_t if a CUDA call failed (1000+CUresult for driver errors).
  *
+ * Padded batches (the *_varlen entry points): B clouds of different sizes are held as [B, N_max, ...] with lengths [B]
+ * (int32, DEVICE): cloud b's points are its rows n < lengths[b], later rows are padding that is never read.  Precondition:
+ * 1 <= lengths[b] <= N_max (plus the call's own lower bound).  Kernels clamp each length into [0, N_max], so nothing past
+ * N_max is read or written whatever lengths holds, but the results for an out-of-range length are unspecified.
+ *
  * "split-bf16" operands: two bf16 planes [2][rows][row_stride] with x ~= hi + lo (|err| <= 2^-17 |x|);
  * plane 0 = hi, plane 1 = lo, lo plane `plane_stride` elements after the hi plane.
  */
@@ -42,6 +47,14 @@ typedef struct CUstream_st* cudaStream_t;
 size_t psam_fps_workspace_bytes(int B, int N, int G);
 int psam_fps_f32(const float* xyz, int B, int N, int G, long long* idx_out, float* centers_out, void* workspace,
                  cudaStream_t stream);
+/* psam_fps_f32 on a padded batch: xyz [B, N_max, 3], lengths [B].  Cloud b samples among its
+ * first lengths[b] points and its slots 0 .. min(G, lengths[b]) - 1 are bit-identical to psam_fps_f32 on that cloud alone
+ * with G' = min(G, lengths[b]) (greedy FPS is prefix-consistent): the tie-break block size T is derived from lengths[b],
+ * not from N_max.  Slots lengths[b] .. G-1 repeat sample 0 (index 0, centre xyz[b, 0]).  G may exceed N_max.  The cluster
+ * plan and the workspace come from N_max (psam_fps_workspace_bytes(B, N_max, G)); the result does not depend on them.
+ * Padded-batch rules as stated at the top of this header. */
+int psam_fps_varlen_f32(const float* xyz, const int* lengths, int B, int N_max, int G, long long* idx_out, float* centers_out,
+                        void* workspace, cudaStream_t stream);
 
 /* K nearest keys of every query (exact, direct-difference squared distance, ties by lower index),
  * sorted by (distance, index).  Replaces knn_points = torch.cdist + torch.topk
@@ -49,6 +62,13 @@ int psam_fps_f32(const float* xyz, int B, int N, int G, long long* idx_out, floa
  * idx_out [B,Q,K] int64, d2_out [B,Q,K] squared distances (may be NULL). */
 int psam_knn_f32(const float* query, const float* key, int B, int Q, int N, int K, long long* idx_out, float* d2_out,
                  cudaStream_t stream);
+/* psam_knn_f32 on a padded batch: key [B, N_max, 3], lengths [B]; the keys of cloud b are its first lengths[b] rows, and
+ * every query row's indices and distances equal psam_knn_f32 on the unpadded cloud bit for bit, ties included.  Query rows
+ * are not limited (query [B, Q, 3]): the outputs of padded query rows are valid results for those points, and callers
+ * ignore them.  Precondition: K <= lengths[b] (a length below K is treated as K).  K <= N_max.
+ * Padded-batch rules as stated at the top of this header. */
+int psam_knn_varlen_f32(const float* query, const float* key, const int* lengths, int B, int Q, int N_max, int K,
+                        long long* idx_out, float* d2_out, cudaStream_t stream);
 
 /* Group-feature gather: groups[b2,g,k,:] = [(xyz[b,idx]-centers[b,g])/radius, feats[b2,idx,0:C]], b=b2/rep.
  * Replaces the fancy-index gathers of KNNGrouper.forward (common.py:99-120) and
@@ -346,6 +366,16 @@ int psam_mask_candidates_batched_f32(const float* logits, const float* iou_preds
                                      float mask_threshold, float stability_offset, float pred_iou_thresh, float stability_thresh,
                                      int min_area, long long base, long long cloud_stride, int W, uint32_t* bits, int* area,
                                      float* stability, float* score, cudaStream_t stream);
+/* psam_mask_candidates_batched_f32 on a padded batch: rows have N_max logits (the row stride), of which cloud b's first
+ * lengths[b] are its points.  Only those are counted and packed (bits past lengths[b] are 0, so psam_mask_nms_batched stays
+ * exact with W = ceil(N_max/32)), and the slots of prompts j >= min(P, lengths[b]) (prompt j owns slots j * C .. j * C + C-1
+ * of the cloud's block, counted from the block start, base included) score -inf.  Every cloud's other slots equal
+ * psam_mask_candidates_f32 on its own unpadded rows.  P >= 0; the other rules are psam_mask_candidates_batched_f32's.
+ * Padded-batch rules as stated at the top of this header. */
+int psam_mask_candidates_varlen_f32(const float* logits, const float* iou_preds, const int* lengths, int B, int Zc, int C,
+                                    int N_max, int P, float mask_threshold, float stability_offset, float pred_iou_thresh,
+                                    float stability_thresh, int min_area, long long base, long long cloud_stride, int W,
+                                    uint32_t* bits, int* area, float* stability, float* score, cudaStream_t stream);
 
 /* Greedy mask-IoU non-maximum suppression over K <= 16384 candidate slots of W words each (the output of
  * psam_mask_candidates_f32).  Stands in for the duplicate-removal stage of SamAutomaticMaskGenerator._process_batch /
@@ -409,6 +439,14 @@ size_t psam_mask_regions_batched_workspace_bytes(int B, int K, int N);
 int psam_mask_regions_batched(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* keep,
                               const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out,
                               int* area_out, float* score_out, void* workspace, cudaStream_t stream);
+/* psam_mask_regions_batched on a padded batch: cloud b's working sets (holes, then islands) hold only its points
+ * n < lengths[b], so padding never forms a component; nbr [B, N_max, k1] is psam_knn_varlen_f32's graph (the generator uses
+ * k1 = min(9, lengths[b]) for every cloud).  Each cloud's outputs equal psam_mask_regions on its own cloud; bits past
+ * lengths[b] are 0.  Workspace: psam_mask_regions_batched_workspace_bytes(B, K, N_max).
+ * Padded-batch rules as stated at the top of this header. */
+int psam_mask_regions_varlen(const uint32_t* bits, long long cloud_slots, const int* lengths, int B, int K, int W, int N_max,
+                             const int* keep, const int* keep_count, const long long* nbr, int k1, int min_area,
+                             uint32_t* bits_out, int* area_out, float* score_out, void* workspace, cudaStream_t stream);
 
 /* ---- crop layers of automatic mask generation (SAM's crop_n_layers) ------------------------------ */
 /* Layout.  Layer 0 is the whole cloud.  Layer i >= 1 splits every axis a of the cloud's axis-aligned bounding box

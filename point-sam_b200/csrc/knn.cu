@@ -151,10 +151,21 @@ struct KnnSmem {
 
 constexpr int KNN_TILE_QUADS = 32;  // quads (4 keys) per thread and super-tile: 4 x 32 hit bits = 4 registers per centre
 
-template <int C>
+// Stride of phase A's key sample: expected candidate count ~ K*stride (<= 1024), sample size >= 4K and <= KNN_MAX_SAMPLE.
+// The result never depends on it (the sample only bounds the candidate filter).
+__host__ __device__ __forceinline__ int knn_sample_stride(int N, int K) {
+    int stride = 1;
+    while ((long long)K * stride * 2 <= 1024 && (N + 2 * stride - 1) / (2 * stride) >= 4 * K) stride *= 2;
+    while ((N + stride - 1) / stride > KNN_MAX_SAMPLE) stride *= 2;
+    return stride;
+}
+
+// VARLEN: the keys of cloud b are the first lengths[b] of its Ns rows (clamped to [K, Ns]), with their own sample stride;
+// otherwise every cloud has Ns keys.  Query rows are never limited.
+template <int C, bool VARLEN>
 __global__ void __launch_bounds__(KNN_THREADS)
-knn_kernel(const float* __restrict__ query, const float* __restrict__ key, int Q, int N, int K, int sample_stride,
-           int sample_cap, int cap, long long* __restrict__ idx_out, float* __restrict__ d2_out) {
+knn_kernel(const float* __restrict__ query, const float* __restrict__ key, const int* __restrict__ lengths, int Q, int Ns,
+           int K, int sample_stride_all, int sample_cap, int cap, long long* __restrict__ idx_out, float* __restrict__ d2_out) {
     pdl_prologue();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* s_sample = reinterpret_cast<float*>(smem_raw);       // [sample_cap = 2K]: the final list of the centre being finished
@@ -167,7 +178,9 @@ knn_kernel(const float* __restrict__ query, const float* __restrict__ key, int Q
     __shared__ int s_wcnt[KNN_THREADS / 32];
 
     const int b = blockIdx.y, q0 = blockIdx.x * C, tid = threadIdx.x, lane = tid & 31;
-    key += (size_t)b * N * 3;
+    const int N = VARLEN ? min(max(lengths[b], K), Ns) : Ns;
+    const int sample_stride = VARLEN ? knn_sample_stride(N, K) : sample_stride_all;
+    key += (size_t)b * Ns * 3;
     float cx[C], cy[C], cz[C];
 #pragma unroll
     for (int c = 0; c < C; ++c) {
@@ -759,19 +772,16 @@ extern "C" int psam_nn_distance_f32(const float* query, const float* key, int n1
     return PSAM_OK;
 }
 
-extern "C" int psam_knn_f32(const float* query, const float* key, int B, int Q, int N, int K, long long* idx_out,
-                            float* d2_out, cudaStream_t stream) {
-    using namespace psam;
-    if (!query || !key || !idx_out || B <= 0 || Q <= 0 || N <= 0 || K <= 0 || K > N) return PSAM_ERR_ARG;
+namespace psam {
+
+template <bool VARLEN>
+static int knn_dispatch(const float* query, const float* key, const int* lengths, int B, int Q, int N, int K, long long* idx_out,
+                        float* d2_out, cudaStream_t stream) {
     if (K > 1024) return PSAM_ERR_UNSUPPORTED;
-    // sample stride: expected candidate count ~ K*stride (<= 1024), sample size >= 4K and <= the smem limit
-    int stride = 1;
-    while ((long long)K * stride * 2 <= 1024 && (N + 2 * stride - 1) / (2 * stride) >= 4 * K) stride *= 2;
-    while ((N + stride - 1) / stride > KNN_MAX_SAMPLE) stride *= 2;
-    const int ns = (N + stride - 1) / stride;
-    (void)ns;
+    const int stride = knn_sample_stride(N, K);
     int sample_cap = (2 * K + 3) & ~3;  // scratch for the final (distance, index) list of one centre
-    // candidate capacity per centre: the bound admits ~1.2 K stride keys (sampling std ~ K^-1/2); beyond it the exact fallback runs
+    // candidate capacity per centre: the bound admits ~1.2 K stride keys (sampling std ~ K^-1/2); beyond it the exact fallback runs.
+    // A shorter cloud of a padded batch has a stride no larger than this one's, so the same capacity serves it.
     long long cap = (long long)2 * K * stride;
     if (cap < 1024) cap = 1024;
     if (cap > KNN_MAX_CAP) cap = KNN_MAX_CAP;
@@ -786,9 +796,9 @@ extern "C" int psam_knn_f32(const float* query, const float* key, int B, int Q, 
     const dim3 grid((unsigned)((Q + C - 1) / C), (unsigned)B);
 #define PSAM_KNN_LAUNCH(CC)                                                                                                  \
     do {                                                                                                                     \
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(knn_kernel<CC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));         \
-        PSAM_CUDA_TRY(psam::launch(knn_kernel<CC>, grid, dim3(KNN_THREADS), smem, stream, query, key, Q, N, K, stride,      \
-                                   sample_cap, (int)cap, idx_out, d2_out));                                                 \
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(knn_kernel<CC, VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        PSAM_CUDA_TRY(psam::launch(knn_kernel<CC, VARLEN>, grid, dim3(KNN_THREADS), smem, stream, query, key, lengths, Q, N, \
+                                   K, stride, sample_cap, (int)cap, idx_out, d2_out));                                      \
     } while (0)
     if (C == 4) PSAM_KNN_LAUNCH(4);
     else if (C == 2) PSAM_KNN_LAUNCH(2);
@@ -796,6 +806,20 @@ extern "C" int psam_knn_f32(const float* query, const float* key, int B, int Q, 
 #undef PSAM_KNN_LAUNCH
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
+}
+
+}  // namespace psam
+
+extern "C" int psam_knn_f32(const float* query, const float* key, int B, int Q, int N, int K, long long* idx_out,
+                            float* d2_out, cudaStream_t stream) {
+    if (!query || !key || !idx_out || B <= 0 || Q <= 0 || N <= 0 || K <= 0 || K > N) return PSAM_ERR_ARG;
+    return psam::knn_dispatch<false>(query, key, nullptr, B, Q, N, K, idx_out, d2_out, stream);
+}
+
+extern "C" int psam_knn_varlen_f32(const float* query, const float* key, const int* lengths, int B, int Q, int N_max, int K,
+                                   long long* idx_out, float* d2_out, cudaStream_t stream) {
+    if (!query || !key || !lengths || !idx_out || B <= 0 || Q <= 0 || N_max <= 0 || K <= 0 || K > N_max) return PSAM_ERR_ARG;
+    return psam::knn_dispatch<true>(query, key, lengths, B, Q, N_max, K, idx_out, d2_out, stream);
 }
 
 extern "C" int psam_group_gather_f32(const float* xyz, const float* feats, const float* centers,

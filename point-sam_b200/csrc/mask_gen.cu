@@ -33,27 +33,31 @@ __device__ __forceinline__ bool candidate_survives(float iou, float stab, int ar
     return area >= min_area && area >= 1;
 }
 
-template <bool VEC>
+// VARLEN: rows have Ns logits of which cloud b's first lengths[b] (clamped to [0, Ns]) are points; only those are counted and
+// packed (later bits are 0), and the slots of prompts past min(P, lengths[b]) (slot / C) score -inf.  Otherwise N = Ns.
+template <bool VEC, bool VARLEN>
 __global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const float* __restrict__ logits,
-                                                                       const float* __restrict__ iou_preds, int N,
+                                                                       const float* __restrict__ iou_preds, int Ns,
                                                                        float thr, float thr_hi, float thr_lo, float iou_t,
                                                                        float stab_t, int min_area, long long base,
                                                                        int rows_per_cloud, long long cloud_stride, int W,
+                                                                       const int* __restrict__ lengths, int P, int C,
                                                                        uint32_t* __restrict__ bits, int* __restrict__ area_out,
                                                                        float* __restrict__ stab_out, float* __restrict__ score_out) {
     psam::pdl_prologue();
     constexpr int U = 4;  // warp iterations whose loads are issued together
     const int row = blockIdx.x;
-    const float* rp = logits + (size_t)row * N;
+    const float* rp = logits + (size_t)row * Ns;
     const int cloud = row / rows_per_cloud;  // rows of cloud b are b * rows_per_cloud .. (b + 1) * rows_per_cloud
     const long long slot = cloud * cloud_stride + base + (row - cloud * rows_per_cloud);
+    const int N = VARLEN ? min(max(lengths[cloud], 0), Ns) : Ns;
     uint32_t* bp = bits + (size_t)slot * W;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     int n_area = 0, n_hi = 0, n_lo = 0;
     if (VEC) {
         // a warp iteration covers 128 points = 4 words; lane l holds points 4l..4l+3 of it
         const float4* rp4 = reinterpret_cast<const float4*>(rp);
-        const int n4 = N >> 2;
+        const int n4 = VARLEN ? (N + 3) >> 2 : N >> 2;  // VEC needs Ns % 4 == 0, so a cloud's last quad is inside its row
         const int iters = (W + 3) >> 2;
         for (int it0 = warp * U; it0 < iters; it0 += nw * U) {
             float4 v[U];
@@ -71,7 +75,7 @@ __global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const flo
                 uint32_t nib = 0;
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    if (in) {
+                    if (in && (!VARLEN || (it * 32 + lane) * 4 + e < N)) {
                         nib |= (uint32_t)(x[e] > thr) << e;
                         n_hi += x[e] > thr_hi;
                         n_lo += x[e] > thr_lo;
@@ -130,7 +134,9 @@ __global__ void __launch_bounds__(kCandThreads) mask_candidates_kernel(const flo
         const float iou = iou_preds[row];
         area_out[slot] = a;
         stab_out[slot] = stab;
-        score_out[slot] = candidate_survives(iou, stab, a, iou_t, stab_t, min_area) ? iou : -INFINITY;
+        bool keep = candidate_survives(iou, stab, a, iou_t, stab_t, min_area);
+        if constexpr (VARLEN) keep = keep && (slot - cloud * cloud_stride) / C < min(P, N);
+        score_out[slot] = keep ? iou : -INFINITY;
     }
 }
 
@@ -436,18 +442,19 @@ __device__ __forceinline__ int region_root(const int* par, int i) { return par[i
 
 // Items it = b * K + p of B clouds: cloud b's candidates start at bits + b * cloud_slots * W, its graph at nbr + b * N * k1,
 // its keep list and outputs at b * K; its count is keep_count[b].
-template <bool SMEM>
+// VARLEN: cloud b's working sets hold only its first lengths[b] points (clamped to [0, N]); N stays the stride of the graph.
+template <bool SMEM, bool VARLEN>
 __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint32_t* __restrict__ bits, long long cloud_slots, int B,
-                                                                      int K, int W, int N, const int* __restrict__ keep,
+                                                                      int K, int W, int Ns, const int* __restrict__ lengths,
+                                                                      const int* __restrict__ keep,
                                                                       const int* __restrict__ keep_count,
                                                                       const long long* __restrict__ nbr, int k1, int min_area,
                                                                       uint32_t* __restrict__ bits_out, int* __restrict__ area_out,
                                                                       float* __restrict__ score_out, int* __restrict__ workspace) {
     psam::pdl_prologue();
     extern __shared__ __align__(16) uint32_t region_smem[];
-    const int Wn = (N + 31) >> 5;
     uint32_t* sw = region_smem;
-    int* par = SMEM ? reinterpret_cast<int*>(region_smem + ((Wn + 3) & ~3)) : workspace + (size_t)blockIdx.x * N;
+    int* par = SMEM ? reinterpret_cast<int*>(region_smem + ((((Ns + 31) >> 5) + 3) & ~3)) : workspace + (size_t)blockIdx.x * Ns;
     __shared__ int changed, any_small, area_red;
     __shared__ unsigned long long best;  // (size << 32) | ~root: the largest component, smallest root on equal sizes
     const int lane = threadIdx.x & 31;
@@ -458,8 +465,10 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
             if (threadIdx.x == 0) score_out[it] = -INFINITY;
             continue;
         }
+        const int N = VARLEN ? min(max(lengths[b], 0), Ns) : Ns;
+        const int Wn = (N + 31) >> 5;
         const uint32_t* src = bits + ((size_t)b * cloud_slots + keep[it]) * W;
-        const long long* cnbr = nbr + (size_t)b * N * k1;
+        const long long* cnbr = nbr + (size_t)b * Ns * k1;
         for (int w = threadIdx.x; w < Wn; w += blockDim.x) {
             const int tail = N - 32 * w;
             sw[w] = tail >= 32 ? src[w] : src[w] & ((1u << tail) - 1u);
@@ -523,23 +532,45 @@ __global__ void __launch_bounds__(kRegionThreads) mask_regions_kernel(const uint
 
 }  // namespace
 
-extern "C" int psam_mask_candidates_batched_f32(const float* logits, const float* iou_preds, int B, int Zc, int C, int N,
-                                                float mask_threshold, float stability_offset, float pred_iou_thresh,
-                                                float stability_thresh, int min_area, long long base, long long cloud_stride,
-                                                int W, uint32_t* bits, int* area, float* stability, float* score,
-                                                cudaStream_t stream) {
+namespace {
+
+int mask_candidates_launch(const float* logits, const float* iou_preds, int B, int Zc, int C, int N, const int* lengths, int P,
+                           float mask_threshold, float stability_offset, float pred_iou_thresh, float stability_thresh,
+                           int min_area, long long base, long long cloud_stride, int W, uint32_t* bits, int* area,
+                           float* stability, float* score, cudaStream_t stream) {
     if (!logits || !iou_preds || !bits || !area || !stability || !score) return PSAM_ERR_ARG;
     if (B <= 0 || Zc <= 0 || C <= 0 || N <= 0 || base < 0 || W < psam::ceil_div(N, 32)) return PSAM_ERR_ARG;
     if ((long long)B * Zc * C > 0x7fffffffLL) return PSAM_ERR_ARG;
     if (B > 1 && cloud_stride < base + (long long)Zc * C) return PSAM_ERR_ARG;  // the clouds' slot blocks must not overlap
     const float thr_hi = mask_threshold + stability_offset, thr_lo = mask_threshold - stability_offset;
     const bool vec = (N % 4 == 0) && (reinterpret_cast<uintptr_t>(logits) % 16 == 0);
-    auto kernel = vec ? mask_candidates_kernel<true> : mask_candidates_kernel<false>;
+    auto kernel = lengths ? (vec ? mask_candidates_kernel<true, true> : mask_candidates_kernel<false, true>)
+                          : (vec ? mask_candidates_kernel<true, false> : mask_candidates_kernel<false, false>);
     PSAM_CUDA_TRY(psam::launch(kernel, dim3(B * Zc * C), dim3(kCandThreads), (size_t)0, stream, logits, iou_preds, N, mask_threshold,
-                               thr_hi, thr_lo, pred_iou_thresh, stability_thresh, min_area, base, Zc * C, cloud_stride, W, bits,
-                               area, stability, score));
+                               thr_hi, thr_lo, pred_iou_thresh, stability_thresh, min_area, base, Zc * C, cloud_stride, W, lengths,
+                               P, C, bits, area, stability, score));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
+}
+
+}  // namespace
+
+extern "C" int psam_mask_candidates_batched_f32(const float* logits, const float* iou_preds, int B, int Zc, int C, int N,
+                                                float mask_threshold, float stability_offset, float pred_iou_thresh,
+                                                float stability_thresh, int min_area, long long base, long long cloud_stride,
+                                                int W, uint32_t* bits, int* area, float* stability, float* score,
+                                                cudaStream_t stream) {
+    return mask_candidates_launch(logits, iou_preds, B, Zc, C, N, nullptr, 0, mask_threshold, stability_offset, pred_iou_thresh,
+                                  stability_thresh, min_area, base, cloud_stride, W, bits, area, stability, score, stream);
+}
+
+extern "C" int psam_mask_candidates_varlen_f32(const float* logits, const float* iou_preds, const int* lengths, int B, int Zc, int C,
+                                               int N_max, int P, float mask_threshold, float stability_offset, float pred_iou_thresh,
+                                               float stability_thresh, int min_area, long long base, long long cloud_stride, int W,
+                                               uint32_t* bits, int* area, float* stability, float* score, cudaStream_t stream) {
+    if (!lengths || P < 0) return PSAM_ERR_ARG;
+    return mask_candidates_launch(logits, iou_preds, B, Zc, C, N_max, lengths, P, mask_threshold, stability_offset, pred_iou_thresh,
+                                  stability_thresh, min_area, base, cloud_stride, W, bits, area, stability, score, stream);
 }
 
 extern "C" int psam_mask_candidates_f32(const float* logits, const float* iou_preds, int Z, int C, int N, float mask_threshold,
@@ -602,9 +633,11 @@ extern "C" size_t psam_mask_regions_batched_workspace_bytes(int B, int K, int N)
 
 extern "C" size_t psam_mask_regions_workspace_bytes(int K, int N) { return psam_mask_regions_batched_workspace_bytes(1, K, N); }
 
-extern "C" int psam_mask_regions_batched(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* keep,
-                                         const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out,
-                                         int* area_out, float* score_out, void* workspace, cudaStream_t stream) {
+namespace {
+
+int mask_regions_launch(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* lengths, const int* keep,
+                        const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out, int* area_out,
+                        float* score_out, void* workspace, cudaStream_t stream) {
     if (!keep_count || !nbr || !workspace) return PSAM_ERR_ARG;
     if (K > 0 && (!bits || !keep || !bits_out || !area_out || !score_out)) return PSAM_ERR_ARG;
     if (N <= 0 || N > kRegionMaxN || W < psam::ceil_div(N, 32) || k1 < 1 || k1 > N || K < 0 || K > kNmsMaxK || min_area < 1)
@@ -622,17 +655,35 @@ extern "C" int psam_mask_regions_batched(const uint32_t* bits, long long cloud_s
     const size_t words = (size_t)(psam::ceil_div(N, 32) + 3) / 4 * 4 * sizeof(uint32_t);
     if (N <= kRegionSmemMaxN) {
         const size_t smem = words + (size_t)N * sizeof(int);
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<true>, dim3(grid), dim3(kRegionThreads), smem, stream, bits, cloud_slots, B, K,
-                                   W, N, keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out, (int*)nullptr));
+        auto kernel = lengths ? mask_regions_kernel<true, true> : mask_regions_kernel<true, false>;
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PSAM_CUDA_TRY(psam::launch(kernel, dim3(grid), dim3(kRegionThreads), smem, stream, bits, cloud_slots, B, K, W, N, lengths, keep,
+                                   keep_count, nbr, k1, min_area, bits_out, area_out, score_out, (int*)nullptr));
     } else {
-        PSAM_CUDA_TRY(cudaFuncSetAttribute(mask_regions_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)words));
-        PSAM_CUDA_TRY(psam::launch(mask_regions_kernel<false>, dim3(grid), dim3(kRegionThreads), words, stream, bits, cloud_slots, B,
-                                   K, W, N, keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out,
-                                   static_cast<int*>(workspace)));
+        auto kernel = lengths ? mask_regions_kernel<false, true> : mask_regions_kernel<false, false>;
+        PSAM_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)words));
+        PSAM_CUDA_TRY(psam::launch(kernel, dim3(grid), dim3(kRegionThreads), words, stream, bits, cloud_slots, B, K, W, N, lengths,
+                                   keep, keep_count, nbr, k1, min_area, bits_out, area_out, score_out, static_cast<int*>(workspace)));
     }
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
+}
+
+}  // namespace
+
+extern "C" int psam_mask_regions_batched(const uint32_t* bits, long long cloud_slots, int B, int K, int W, int N, const int* keep,
+                                         const int* keep_count, const long long* nbr, int k1, int min_area, uint32_t* bits_out,
+                                         int* area_out, float* score_out, void* workspace, cudaStream_t stream) {
+    return mask_regions_launch(bits, cloud_slots, B, K, W, N, nullptr, keep, keep_count, nbr, k1, min_area, bits_out, area_out,
+                               score_out, workspace, stream);
+}
+
+extern "C" int psam_mask_regions_varlen(const uint32_t* bits, long long cloud_slots, const int* lengths, int B, int K, int W, int N_max,
+                                        const int* keep, const int* keep_count, const long long* nbr, int k1, int min_area,
+                                        uint32_t* bits_out, int* area_out, float* score_out, void* workspace, cudaStream_t stream) {
+    if (!lengths) return PSAM_ERR_ARG;
+    return mask_regions_launch(bits, cloud_slots, B, K, W, N_max, lengths, keep, keep_count, nbr, k1, min_area, bits_out, area_out,
+                               score_out, workspace, stream);
 }
 
 extern "C" int psam_mask_regions(const uint32_t* bits, int K, int W, int N, const int* keep, const int* keep_count,

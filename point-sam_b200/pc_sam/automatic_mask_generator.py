@@ -21,6 +21,13 @@ all B clouds; each decode batch covers the same prompt range of every cloud (``p
 small-region launch covers all B clouds, each owning a block of ``points_per_cloud * 3`` candidate slots.  One host read
 covers all B kept counts.  Generation on one cloud is the case B = 1 of the same code.
 
+Clouds of different sizes (a sequence of [N_b, 3] tensors) run the same path on a padded batch [B, N_max, 3] with lengths
+[B] on the device (``ops.pad_clouds``).  Farthest-point sampling, the kNN searches, the candidate pass and the small-region
+pass stay inside each cloud's own points, so every cloud gets generate_packed's masks; cloud b uses min(points_per_cloud,
+N_b) prompts as generate_packed does (its other prompt slots score -inf).  Everything between the tokenizer and the mask
+dot sees G patches per cloud or independent point rows, and the decoder also computes logits for the padded rows: that
+cost grows with B * N_max - sum(N_b).  Group clouds of similar sizes to keep it small.
+
 Crop layers (keyword ``crop_n_layers > 0``, SAM's zoomed crops for large scenes): ``psam_crop_layout_f32`` splits the cloud's
 bounding box into 2^i x 2^i x 2^i overlapping boxes on layer i and counts their points; the host reads the counts once.
 Layer 0 runs steps 1-5 on the cloud as given.  Every other crop with at least as many points as the tokenizer's first-level
@@ -31,12 +38,12 @@ whole cloud, and ``psam_mask_nms`` with score = layer and ``crop_nms_thresh`` me
 then runs on the merged set.  The host synchronises twice: the counts, and the final read.
 
 Memory: each batch of Z = points_per_batch prompts decodes Z rows of N points (with B clouds, points_per_batch // B
-prompts of each cloud).  The split-bf16 input of the last upscaling Linear is Z*N*Du*4 bytes (Du = 256 for PointCloudSAM, 128 for PointCloudSAMHier): about 2 GB at Z = 64,
+prompts of each cloud; N = N_max for clouds of different sizes).  The split-bf16 input of the last upscaling Linear is Z*N*Du*4 bytes (Du = 256 for PointCloudSAM, 128 for PointCloudSAMHier): about 2 GB at Z = 64,
 N = 32768, Du = 256.  Lower points_per_batch to trade speed for memory.
 """
 from __future__ import annotations
 
-from typing import Dict, List, NamedTuple, Tuple
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -55,7 +62,7 @@ class DecodePlan(NamedTuple):
 
 
 def plan_decode(B: int, P: int, N: int, points_per_batch: int) -> DecodePlan:
-    """Decode batches for B clouds of N points with P prompts each.  A batch covers prompts [s, e) of every cloud, row
+    """Decode batches for B clouds of N points (N_max for a padded batch of clouds of different sizes) with P prompts each.  A batch covers prompts [s, e) of every cloud, row
     b * (e - s) + j of the decoder for prompt s + j of cloud b.  Zc = max(1, points_per_batch // B) keeps points_per_batch
     rows per batch (the memory bound of the module docstring); the last batch may be short.  Raises ValueError when even
     one prompt per cloud needs more than DECODE_MAX_ROW_TILES row tiles (ceil(B * N / 128)): fewer clouds per call fit."""
@@ -143,15 +150,17 @@ class PointCloudMaskGenerator:
                      "region_score", "region_keep")
         return {k: (v[b] if k in per_cloud else v[b:b + 1] if k in ("keep_count", "region_count") else v) for k, v in st.items()}
 
-    def _generate_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None) -> Dict[str, torch.Tensor]:
+    def _generate_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, P: int, edge=None,
+                        lengths: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
         """Generation on B clouds [B, N, 3] (whole clouds, or one crop's renormalised cloud, B = 1): one encode, P FPS
         prompts per cloud, multimask decode in the batches of plan_decode with one candidate launch each, the crop's edge
         filter when `edge` is given (B = 1), mask NMS per cloud in one go.  Cloud b owns candidate slots b * P * C .. of
-        bits [B, P*C, W]; keep [B, P*C] holds slots within the cloud, keep_count [B]."""
+        bits [B, P*C, W]; keep [B, P*C] holds slots within the cloud, keep_count [B].  lengths [B] (device): padded clouds,
+        cloud b's first lengths[b] points with min(P, lengths[b]) prompts."""
         m, dev, (B, N, _) = self.model, xyz.device, xyz.shape
         plan = plan_decode(B, P, N, self.points_per_batch)
-        enc = m._encode(xyz, rgb)
-        point_index, centers = ops.fps(xyz, P)
+        enc = m._encode(xyz, rgb) if lengths is None else m._encode(xyz, rgb, lengths)
+        point_index, centers = ops.fps(xyz, P, lengths=lengths)
         labels = torch.ones((B * plan.rows, 1), dtype=torch.int64, device=dev)
         cand, C = None, None
         for s, e in plan.batches:
@@ -166,7 +175,7 @@ class PointCloudMaskGenerator:
             ops.mask_candidates_batched(masks, iou, B, mask_threshold=self.mask_threshold,
                                         stability_offset=self.stability_score_offset, pred_iou_thresh=self.pred_iou_thresh,
                                         stability_thresh=self.stability_score_thresh, min_area=self.min_mask_area, out=cand,
-                                        base=s * C)
+                                        base=s * C, lengths=lengths, num_prompts=P)
         bits, area, stab, score = cand
         if edge is not None:
             ops.crop_edge_filter(bits[0], score[0], edge)
@@ -179,11 +188,13 @@ class PointCloudMaskGenerator:
         return self._cloud_state(self._generate_batch(xyz, rgb, P, edge), 0)
 
     def _regions(self, xyz: torch.Tensor, bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor,
-                 area: int) -> Dict[str, torch.Tensor]:
+                 area: int, lengths: Optional[torch.Tensor] = None, min_points: int = 0) -> Dict[str, torch.Tensor]:
         """The small-region stage on B clouds xyz [B, N, 3]: kept masks keep [B, K] (keep_count [B]) of bits [B, K', W];
-        one kNN launch, one region launch, then mask NMS per cloud in one go."""
-        nbr, _ = ops.knn(xyz, xyz, min(self.region_neighbors + 1, xyz.shape[1]))
-        rbits, rarea, rscore = ops.mask_regions_batched(bits, keep, keep_count, nbr, area)
+        one kNN launch, one region launch, then mask NMS per cloud in one go.  lengths [B] (device): padded clouds, the
+        smallest of min_points points."""
+        k1 = min(self.region_neighbors + 1, xyz.shape[1] if lengths is None else min_points)
+        nbr, _ = ops.knn(xyz, xyz, k1, lengths=lengths)
+        rbits, rarea, rscore = ops.mask_regions_batched(bits, keep, keep_count, nbr, area, lengths=lengths)
         rkeep, rcount = ops.mask_nms_batched(rbits, rarea, rscore, self.mask_nms_thresh)
         return dict(region_bits=rbits, region_area=rarea, region_score=rscore, region_keep=rkeep, region_count=rcount)
 
@@ -264,12 +275,17 @@ class PointCloudMaskGenerator:
         if xyz.shape[:2] != rgb.shape[:2]:
             raise ValueError("xyz and rgb must have the same number of clouds and points")
 
-    def _enqueue_clouds(self, xyz: torch.Tensor, rgb: torch.Tensor, region_area: int) -> Dict[str, torch.Tensor]:
-        """Generation and (region_area > 0) the small-region stage on B validated clouds [B, N, 3], batched state."""
+    def _enqueue_clouds(self, xyz: torch.Tensor, rgb: torch.Tensor, region_area: int, lengths: Optional[torch.Tensor] = None,
+                        sizes: Optional[List[int]] = None) -> Dict[str, torch.Tensor]:
+        """Generation and (region_area > 0) the small-region stage on B validated clouds [B, N, 3], batched state.  lengths
+        (device) and sizes (host): a padded batch of clouds of N_b = sizes[b] points."""
         with torch.no_grad():
-            st = self._generate_batch(xyz, rgb, min(self.points_per_cloud, xyz.shape[1]))
+            st = self._generate_batch(xyz, rgb, min(self.points_per_cloud, xyz.shape[1]), lengths=lengths)
             if region_area > 0:
-                st.update(self._regions(xyz, st["bits"], st["keep"], st["keep_count"], region_area))
+                st.update(self._regions(xyz, st["bits"], st["keep"], st["keep_count"], region_area, lengths=lengths,
+                                        min_points=min(sizes) if sizes else 0))
+        if sizes is not None:
+            st["sizes"] = sizes
         return st
 
     def _enqueue(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
@@ -292,13 +308,23 @@ class PointCloudMaskGenerator:
                 st.update(self._cloud_state(self._regions(xyz, st["bits"][None], st["keep"][None], st["keep_count"], region_area), 0))
         return st
 
-    def _enqueue_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
-        """Enqueue the generation of B clouds [B, N, 3] on the current stream; nothing here waits for the device."""
+    def _enqueue_batch(self, xyz: Union[torch.Tensor, Sequence[torch.Tensor]], rgb: Union[torch.Tensor, Sequence[torch.Tensor]], *,
+                       min_mask_region_area: int = 0) -> Dict[str, torch.Tensor]:
+        """Enqueue the generation of B clouds [B, N, 3], or of a sequence of B clouds [N_b, 3] as one padded batch, on the
+        current stream; nothing here waits for the device."""
         region_area = self._region_area(min_mask_region_area)
         self._check_model()
-        xyz, rgb = self._clouds(xyz, "xyz"), self._clouds(rgb, "rgb")
-        self._same_points(xyz, rgb)
-        return self._enqueue_clouds(xyz, rgb, region_area)
+        if torch.is_tensor(xyz):
+            xyz, rgb = self._clouds(xyz, "xyz"), self._clouds(rgb, "rgb")
+            self._same_points(xyz, rgb)
+            return self._enqueue_clouds(xyz, rgb, region_area)
+        if torch.is_tensor(rgb):
+            raise ValueError("xyz and rgb must both be [B, N, 3] tensors or both sequences of [N_b, 3] tensors")
+        sizes = self.model.varlen_clouds(xyz, rgb)
+        if any(t.shape[1] != 3 for t in rgb):
+            raise ValueError("rgb must hold [N_b, 3] tensors")
+        xyz, rgb, lengths = ops.pad_clouds(xyz, rgb)
+        return self._enqueue_clouds(xyz, rgb, region_area, lengths, sizes)
 
     @staticmethod
     def _read_counts(st: Dict[str, torch.Tensor]) -> List[int]:
@@ -347,8 +373,12 @@ class PointCloudMaskGenerator:
 
     @classmethod
     def _finish_batch(cls, st: Dict[str, torch.Tensor]) -> List[Dict[str, torch.Tensor]]:
-        """Every cloud's output from a batched state (_enqueue_batch), after one host synchronisation for all of them."""
-        return [cls._select(cls._cloud_state(st, b), n) for b, n in enumerate(cls._read_counts(st))]
+        """Every cloud's output from a batched state (_enqueue_batch), after one host synchronisation for all of them.  The
+        masks of a padded batch keep the ceil(N_b / 32) words of their own cloud (the later ones are zero)."""
+        outs = [cls._select(cls._cloud_state(st, b), n) for b, n in enumerate(cls._read_counts(st))]
+        for out, n in zip(outs, st.get("sizes", ())):
+            out["bits"] = out["bits"][:, :ops.mask_words(n)].contiguous()
+        return outs
 
     def generate_packed(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0, crop_n_layers: int = 0,
                         crop_nms_thresh: float = 0.7, crop_overlap_ratio: float = 512 / 1500,
@@ -374,13 +404,15 @@ class PointCloudMaskGenerator:
                                           crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
                                           crop_n_points_downscale_factor=crop_n_points_downscale_factor))
 
-    def generate_packed_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *,
-                              min_mask_region_area: int = 0) -> List[Dict[str, torch.Tensor]]:
-        """generate_packed on B clouds of the same N at once: xyz / rgb [B, N, 3] CUDA tensors, xyz normalised to [-1, 1].
-        Returns B dicts with generate_packed's fields, dtypes, order and meaning for each cloud.  The clouds share one encode,
-        the decode batches (points_per_batch // B prompts of every cloud each) and every post-processing launch, and the host
-        synchronises once for all of them; a cloud outside [-1, 1] raises ValueError for the whole call.  Crop layers are
-        not supported here (crops of different clouds differ in size): use generate_packed per cloud."""
+    def generate_packed_batch(self, xyz: Union[torch.Tensor, Sequence[torch.Tensor]], rgb: Union[torch.Tensor, Sequence[torch.Tensor]],
+                              *, min_mask_region_area: int = 0) -> List[Dict[str, torch.Tensor]]:
+        """generate_packed on B clouds at once: xyz / rgb [B, N, 3] CUDA tensors, or sequences of B CUDA tensors [N_b, 3] for
+        clouds of different sizes; xyz normalised to [-1, 1].  Returns B dicts with generate_packed's fields, dtypes, order
+        and meaning for each cloud (bits [K, ceil(N_b / 32)]).  The clouds share one encode, the decode batches
+        (points_per_batch // B prompts of every cloud each) and every post-processing launch, and the host synchronises
+        once for all of them; a cloud outside [-1, 1] raises ValueError for the whole call.  Clouds of different sizes are
+        padded to the largest (module docstring): the decoder's work grows with the padding.  Crop layers are not supported
+        here (crops of different clouds differ in size): use generate_packed per cloud."""
         return self._finish_batch(self._enqueue_batch(xyz, rgb, min_mask_region_area=min_mask_region_area))
 
     @staticmethod
@@ -406,7 +438,13 @@ class PointCloudMaskGenerator:
                                                   crop_nms_thresh=crop_nms_thresh, crop_overlap_ratio=crop_overlap_ratio,
                                                   crop_n_points_downscale_factor=crop_n_points_downscale_factor), N)
 
-    def generate_batch(self, xyz: torch.Tensor, rgb: torch.Tensor, *, min_mask_region_area: int = 0) -> List[List[Dict]]:
-        """generate on B clouds [B, N, 3] at once (see generate_packed_batch): one record list per cloud."""
-        N = self._clouds(xyz, "xyz").shape[1]
-        return [self._records(out, N) for out in self.generate_packed_batch(xyz, rgb, min_mask_region_area=min_mask_region_area)]
+    def generate_batch(self, xyz: Union[torch.Tensor, Sequence[torch.Tensor]], rgb: Union[torch.Tensor, Sequence[torch.Tensor]], *,
+                       min_mask_region_area: int = 0) -> List[List[Dict]]:
+        """generate on B clouds [B, N, 3], or a sequence of clouds [N_b, 3], at once (see generate_packed_batch): one record
+        list per cloud, whose segmentations have the cloud's own N_b points."""
+        if torch.is_tensor(xyz):
+            sizes = [self._clouds(xyz, "xyz").shape[1]] * xyz.shape[0]
+        else:
+            sizes = [int(t.shape[0]) for t in xyz]
+        outs = self.generate_packed_batch(xyz, rgb, min_mask_region_area=min_mask_region_area)
+        return [self._records(out, n) for out, n in zip(outs, sizes)]

@@ -4,16 +4,16 @@
 All computation runs in the sm_100a kernels behind ``psam_b200`` (no CPU / PyTorch fallback)."""
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
 
-from psam_b200 import engine
+from psam_b200 import engine, ops
 
 from .common import batch_index_select, repeat_interleave
 from .mask_decoder import AuxInputs, MaskDecoder
-from .pc_encoder import PointCloudEncoder
+from .pc_encoder import PatchEmbedNN, PointCloudEncoder
 from .prompt_encoder import MaskEncoder, PointEncoder
 
 
@@ -31,8 +31,15 @@ class PointCloudSAM(nn.Module):
         self._cloud_key = None
 
     # ------------------------------------------------------------------------------------------
-    def _encode(self, coords, features):
-        pc_embeddings, patches = self.pc_encoder(coords, features)
+    def _run_encoder(self, coords, features, lengths):
+        if lengths is None:
+            return self.pc_encoder(coords, features)
+        return engine.run_pc_encoder(self.pc_encoder, coords, features, lengths=lengths)
+
+    def _encode(self, coords, features, lengths=None):
+        """lengths [B] int32 (device): coords / features are padded clouds (ops.pad_clouds), cloud b its first lengths[b]
+        points; the caller has checked every lengths[b] >= the first-level num_groups (varlen_clouds)."""
+        pc_embeddings, patches = self._run_encoder(coords, features, lengths)
         centers = patches["centers"]
         aux = AuxInputs(coords=coords, features=features, centers=centers)
         pc_pe = engine.run_pos_embedding(self.point_encoder.pe_layer, centers, check=False)
@@ -59,6 +66,56 @@ class PointCloudSAM(nn.Module):
     def _group_shape(self) -> tuple:
         g = self.pc_encoder.patch_embed.grouper
         return g.num_groups, g.group_size
+
+    def varlen_clouds(self, coords: Sequence[torch.Tensor], features: Sequence[torch.Tensor]) -> List[int]:
+        """Checks a batch of clouds of different sizes without touching the device and returns their sizes N_b: coords and
+        features are sequences of B >= 1 tensors [N_b, 3] and [N_b, Cf].  A Voronoi tokenizer (PatchEmbedNN) is refused
+        (NotImplementedError: padded points would join its cells' maxima), and so is a cloud smaller than the first-level
+        num_groups (RuntimeError, as for one cloud)."""
+        if isinstance(self.pc_encoder.patch_embed, PatchEmbedNN):
+            raise NotImplementedError("clouds of different sizes need a kNN tokenizer: the Voronoi tokenizer (PatchEmbedNN) "
+                                      "would pool padded points into its cells")
+        if torch.is_tensor(coords) or torch.is_tensor(features):
+            raise TypeError("coords and features must be sequences of [N_b, 3] / [N_b, C] tensors, one per cloud")
+        coords, features = list(coords), list(features)
+        if not coords or len(coords) != len(features):
+            raise ValueError(f"{len(coords)} coordinate and {len(features)} feature tensors: need the same number >= 1")
+        sizes = []
+        for b, (c, f) in enumerate(zip(coords, features)):
+            if c.dim() != 2 or c.shape[1] != 3 or f.dim() != 2 or f.shape[0] != c.shape[0]:
+                raise ValueError(f"cloud {b}: coords {tuple(c.shape)} and features {tuple(f.shape)} must be [N_b, 3] and [N_b, C]")
+            sizes.append(int(c.shape[0]))
+        if min(sizes) < self._group_shape()[0]:
+            raise RuntimeError("sample_farthest_points: number of points must be >= num_samples")
+        return sizes
+
+    def predict_masks_varlen(self, coords: Sequence[torch.Tensor], features: Sequence[torch.Tensor], prompt_coords: torch.Tensor,
+                             prompt_labels: torch.Tensor, prompt_masks: Optional[Sequence[torch.Tensor]] = None,
+                             multimask_output: bool = True) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+        """predict_masks on B clouds of different sizes with one encode and one decode: coords / features are sequences of
+        [N_b, 3] tensors, prompt_coords [B, M, Q, 3], prompt_labels [B, M, Q], prompt_masks None or a sequence of [M, N_b]
+        tensors.  Returns B pairs (masks [M, C, N_b], iou_preds [M, C]).  The clouds are padded to N_max = max N_b
+        (ops.pad_clouds); farthest-point sampling and the kNN grouping stay inside each cloud, and the decoder also computes
+        logits for the padded rows, which are dropped: its cost grows with B * N_max - sum(N_b).  Group clouds of similar
+        sizes to keep that small."""
+        sizes = self.varlen_clouds(coords, features)
+        B = len(sizes)
+        if prompt_coords.dim() != 4 or prompt_coords.shape[0] != B or prompt_labels.shape != prompt_coords.shape[:3]:
+            raise ValueError(f"prompt_coords must be [B={B}, M, Q, 3] and prompt_labels [B, M, Q], got "
+                             f"{tuple(prompt_coords.shape)} and {tuple(prompt_labels.shape)}")
+        M, Q = prompt_coords.shape[1], prompt_coords.shape[2]
+        pm = None
+        if prompt_masks is not None:
+            prompt_masks = list(prompt_masks)
+            if len(prompt_masks) != B or any(t.shape != (M, n) for t, n in zip(prompt_masks, sizes)):
+                raise ValueError(f"prompt_masks must be {B} tensors [M={M}, N_b]")
+            pm = torch.nn.utils.rnn.pad_sequence([t.transpose(0, 1) for t in prompt_masks], batch_first=True)
+            pm = pm.transpose(1, 2).reshape(B * M, -1)
+        xyz, rgb, lengths = ops.pad_clouds(coords, features)
+        enc = self._encode(xyz, rgb, lengths)
+        masks, iou = self._decode(enc, prompt_coords.reshape(B * M, Q, 3), prompt_labels.reshape(B * M, Q), pm,
+                                  bool(multimask_output))
+        return [(masks[b * M:(b + 1) * M, :, :n], iou[b * M:(b + 1) * M]) for b, n in enumerate(sizes)]
 
     def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval):
         from .prompt_sampling import sample_prompts_adapter
@@ -196,8 +253,8 @@ class PointCloudSAMHier(PointCloudSAM):
     this model), and predict_masks / predict_iterative / set_pointcloud run one round of the forward loop body with the
     given prompts (the reference's inherited predict_masks indexes the list of patch levels with a string, pc_sam.py:54)."""
 
-    def _encode(self, coords, features):
-        pc_embeddings, patches = self.pc_encoder(coords, features)
+    def _encode(self, coords, features, lengths=None):
+        pc_embeddings, patches = self._run_encoder(coords, features, lengths)
         p1, p2 = patches
         aux1 = AuxInputs(coords=coords, features=features, centers=p1["centers"])
         aux2 = AuxInputs(coords=p1["centers"], features=p1["embeddings"], centers=p2["centers"])

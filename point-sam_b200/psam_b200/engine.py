@@ -172,18 +172,20 @@ def run_patch_encoder(m, patches: torch.Tensor, want_split: bool = False):
 # ------------------------------------------------------------------------------------------------
 # KNNGrouper, pc_sam/model/common.py:59-123
 # ------------------------------------------------------------------------------------------------
-def run_knn_grouper(g, xyz, features, use_fps=True):
+def run_knn_grouper(g, xyz, features, use_fps=True, lengths=None):
+    """lengths [B] int32 (device): padded clouds, cloud b is its first lengths[b] points (FPS and kNN stay inside it).  The
+    caller guarantees lengths[b] >= num_groups: it cannot be checked here without waiting for the device."""
     xyz32 = xyz.float().contiguous()
     feats = features.float().contiguous()
     B, N, _ = xyz32.shape
     if N < g.num_groups:
         raise RuntimeError("sample_farthest_points: number of points must be >= num_samples")
     if use_fps:
-        fps_idx, centers = ops.fps(xyz32, g.num_groups)
+        fps_idx, centers = ops.fps(xyz32, g.num_groups, lengths=lengths)
     else:  # `xyz` is already FPS-ordered: the first num_groups points are the centres (common.py:93-96)
         fps_idx = torch.arange(g.num_groups, device=xyz.device).expand(B, -1).contiguous()
         centers = xyz32[:, : g.num_groups].contiguous()
-    knn_idx, _ = ops.knn(centers, xyz32, g.group_size)
+    knn_idx, _ = ops.knn(centers, xyz32, g.group_size, lengths=lengths)
     groups = ops.group_gather(xyz32, feats, centers, knn_idx, g.radius,
                               center_idx=fps_idx if g.centralize_features else None)  # common.py:116-118
     return dict(features=groups, centers=centers, knn_idx=knn_idx, fps_idx=fps_idx)
@@ -243,11 +245,12 @@ def _run_res_blocks(blocks, x: torch.Tensor):
         ops.gemm(un, pb.w2, bias=pb.bb2, out_f32=x, resid=x, passes=PASSES)
 
 
-def run_patch_embed_hier(m, coords, features, want_split: bool = False):
+def run_patch_embed_hier(m, coords, features, want_split: bool = False, lengths=None):
     """PatchEmbedHier.forward (pc_encoder.py:200-239): PointNet++-style two-level tokenizer; the second level groups the
     first level's centres (already in FPS order: use_fps=False) with the first level's embeddings as features.
-    want_split: also return the split-bf16 copy of the level-2 embeddings (the operand of patch_proj)."""
-    patches1 = run_knn_grouper(m.grouper1, coords, features)
+    want_split: also return the split-bf16 copy of the level-2 embeddings (the operand of patch_proj).
+    lengths: padded clouds (run_knn_grouper); only the first level sees points, the second sees real centres only."""
+    patches1 = run_knn_grouper(m.grouper1, coords, features, lengths=lengths)
     x1 = run_patch_encoder(m.patch_encoder1, patches1["features"])
     patches1["embeddings"] = x1
     patches2 = run_knn_grouper(m.grouper2, patches1["centers"], x1, use_fps=False)
@@ -596,15 +599,16 @@ def _run_mlp_folded(pb: _PackedBlock, x, xs, st_mid, st_out, M, D, dev, stats=No
         ops.gemm(h, pb.w2, bias=pb.bb2, out_f32=x, resid=x, out_split=xs, stats_out=st_out, passes=PASSES)
 
 
-def run_pc_encoder(enc, coords, features):
+def run_pc_encoder(enc, coords, features, lengths=None):
     """PointCloudEncoder.forward (pc_encoder.py:118-145).  A hierarchical tokenizer (PatchEmbedHier) returns a list of
-    patch dicts: the transformer consumes the last level's embeddings and centres, and the list is returned."""
+    patch dicts: the transformer consumes the last level's embeddings and centres, and the list is returned.
+    lengths: padded clouds, passed to the tokenizer (everything after it sees G real patches per cloud)."""
     pk = _cached(enc, _PackedEncoder)
     if hasattr(enc.patch_embed, "grouper1"):
-        patches, embs = run_patch_embed_hier(enc.patch_embed, coords, features, want_split=True)
+        patches, embs = run_patch_embed_hier(enc.patch_embed, coords, features, want_split=True, lengths=lengths)
         last = patches[-1]
     else:
-        patches = run_knn_grouper(enc.patch_embed.grouper, coords, features)
+        patches = run_knn_grouper(enc.patch_embed.grouper, coords, features, lengths=lengths)
         emb, embs = run_patch_encoder(enc.patch_embed.patch_encoder, patches["features"], want_split=True)
         patches["embeddings"] = emb
         last = patches

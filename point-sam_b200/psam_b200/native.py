@@ -66,6 +66,7 @@ EXPORTS = [
     "psam_mask_regions_workspace_bytes", "psam_mask_regions",
     "psam_mask_candidates_batched_f32", "psam_mask_nms_batched_workspace_bytes", "psam_mask_nms_batched",
     "psam_mask_regions_batched_workspace_bytes", "psam_mask_regions_batched",
+    "psam_fps_varlen_f32", "psam_knn_varlen_f32", "psam_mask_candidates_varlen_f32", "psam_mask_regions_varlen",
     "psam_crop_total", "psam_crop_layout_f32", "psam_crop_gather_workspace_bytes", "psam_crop_gather_f32", "psam_crop_edge_filter",
     "psam_crop_uncrop",
     "psam_mesh_sample_workspace_bytes", "psam_mesh_sample_f32", "psam_mesh_face_centers_f32", "psam_mask_lift", "psam_mask_label_map",
@@ -139,6 +140,10 @@ def lib():
             "psam_mask_candidates_batched_f32": [p, p, i, i, i, i, f, f, f, f, i, ll, ll, i, p, p, p, p, p],
             "psam_mask_nms_batched": [p, p, p, i, i, i, f, p, p, p, p],
             "psam_mask_regions_batched": [p, ll, i, i, i, i, p, p, p, i, i, p, p, p, p, p],
+            "psam_fps_varlen_f32": [p, p, i, i, i, p, p, p, p],
+            "psam_knn_varlen_f32": [p, p, p, i, i, i, i, p, p, p],
+            "psam_mask_candidates_varlen_f32": [p, p, p, i, i, i, i, i, f, f, f, f, i, ll, ll, i, p, p, p, p, p],
+            "psam_mask_regions_varlen": [p, ll, p, i, i, i, i, p, p, p, i, i, p, p, p, p, p],
             "psam_crop_total": [i],
             "psam_crop_layout_f32": [p, i, i, f, p, p, p],
             "psam_crop_gather_f32": [p, p, i, p, i, i, f, i, p, p, p, p, p, p],

@@ -53,23 +53,63 @@ def pack_weight(w: torch.Tensor) -> Split:
 
 
 # ------------------------------------------------------------------------------------------------
-def fps(xyz: torch.Tensor, num_samples: int):
+def pad_clouds(*clouds):
+    """Padded batch of clouds of different sizes: each argument is a sequence of B tensors [N_b, C] (the same N_b for every
+    argument) and becomes one [B, N_max, C] fp32 tensor whose rows n >= N_b are zeros.  Returns the padded tensors followed
+    by lengths [B] int32 on the device (the `lengths` of the varlen ops).  Nothing waits for the device: the lengths are
+    copied from pinned host memory without a synchronisation."""
+    first = clouds[0]
+    if not len(first):
+        raise ValueError("pad_clouds: no clouds")
+    sizes = [int(t.shape[0]) for t in first]
+    for seq in clouds:
+        if len(seq) != len(first) or any(t.dim() != 2 or int(t.shape[0]) != n for t, n in zip(seq, sizes)):
+            raise ValueError(f"pad_clouds: every sequence must hold {len(first)} tensors [N_b, C] with N_b = {sizes}")
+    dev = first[0].device
+    out = [torch.nn.utils.rnn.pad_sequence([t.float() for t in seq], batch_first=True).contiguous() for seq in clouds]
+    host = torch.tensor(sizes, dtype=torch.int32)
+    lengths = (host.pin_memory() if dev.type == "cuda" else host).to(dev, non_blocking=True)
+    return (*out, lengths)
+
+
+def fps(xyz: torch.Tensor, num_samples: int, lengths: Optional[torch.Tensor] = None):
+    """Farthest-point sampling of num_samples centres per cloud of xyz [B, N, 3] -> (idx [B, G] int64, centers [B, G, 3]).
+    lengths [B] int32 (device): cloud b is its first lengths[b] points (psam_fps_varlen_f32); slots past lengths[b] repeat
+    sample 0."""
     B, N, _ = xyz.shape
     idx = torch.empty((B, num_samples), dtype=torch.int64, device=xyz.device)
     centers = torch.empty((B, num_samples, 3), dtype=torch.float32, device=xyz.device)
     nbytes = nv.lib().psam_fps_workspace_bytes(B, N, num_samples)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=xyz.device) if nbytes else None
-    nv.check(nv.lib().psam_fps_f32(nv.ptr(xyz), B, N, num_samples, nv.ptr(idx), nv.ptr(centers), nv.ptr(ws), nv.stream()), "fps")
+    if lengths is None:
+        nv.check(nv.lib().psam_fps_f32(nv.ptr(xyz), B, N, num_samples, nv.ptr(idx), nv.ptr(centers), nv.ptr(ws), nv.stream()), "fps")
+    else:
+        lengths = _lengths(lengths, B, "fps")
+        nv.check(nv.lib().psam_fps_varlen_f32(nv.ptr(xyz), nv.ptr(lengths), B, N, num_samples, nv.ptr(idx), nv.ptr(centers),
+                                              nv.ptr(ws), nv.stream()), "fps")
     return idx, centers
 
 
-def knn(query: torch.Tensor, key: torch.Tensor, k: int, want_d2: bool = False):
+def knn(query: torch.Tensor, key: torch.Tensor, k: int, want_d2: bool = False, lengths: Optional[torch.Tensor] = None):
+    """k nearest keys of every query: query [B, Q, 3], key [B, N, 3] -> (idx [B, Q, k] int64, d2 [B, Q, k] or None).
+    lengths [B] int32 (device): the keys of cloud b are its first lengths[b] rows (psam_knn_varlen_f32)."""
     B, Q, _ = query.shape
     N = key.shape[1]
     idx = torch.empty((B, Q, k), dtype=torch.int64, device=query.device)
     d2 = torch.empty((B, Q, k), dtype=torch.float32, device=query.device) if want_d2 else None
-    nv.check(nv.lib().psam_knn_f32(nv.ptr(query), nv.ptr(key), B, Q, N, k, nv.ptr(idx), nv.ptr(d2), nv.stream()), "knn")
+    if lengths is None:
+        nv.check(nv.lib().psam_knn_f32(nv.ptr(query), nv.ptr(key), B, Q, N, k, nv.ptr(idx), nv.ptr(d2), nv.stream()), "knn")
+    else:
+        lengths = _lengths(lengths, B, "knn")
+        nv.check(nv.lib().psam_knn_varlen_f32(nv.ptr(query), nv.ptr(key), nv.ptr(lengths), B, Q, N, k, nv.ptr(idx), nv.ptr(d2),
+                                              nv.stream()), "knn")
     return idx, d2
+
+
+def _lengths(lengths: torch.Tensor, B: int, what: str) -> torch.Tensor:
+    if lengths.dtype != torch.int32 or lengths.numel() != B:
+        raise ValueError(f"{what}: lengths must be {B} int32 values, got {lengths.numel()} of {lengths.dtype}")
+    return lengths.contiguous()
 
 
 def group_gather(xyz, feats, centers, knn_idx, radius=None, center_idx=None):
@@ -405,10 +445,13 @@ def mask_regions(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tenso
 
 def mask_candidates_batched(logits: torch.Tensor, iou_preds: torch.Tensor, B: int, *, out, base: int = 0,
                             mask_threshold: float = 0.0, stability_offset: float = 1.0, pred_iou_thresh: float = 0.0,
-                            stability_thresh: float = 0.0, min_area: int = 0):
+                            stability_thresh: float = 0.0, min_area: int = 0, lengths: Optional[torch.Tensor] = None,
+                            num_prompts: int = 0):
     """mask_candidates for B clouds in one launch (psam_mask_candidates_batched_f32): logits [B*Zc,C,N], iou_preds [B*Zc,C],
     rows b*Zc .. b*Zc+Zc-1 of cloud b.  Row b*Zc + j, output c fills slot base + j*C + c of cloud b in
-    out = (bits [B,K,W] int32, area [B,K] int32, stability [B,K] fp32, score [B,K] fp32)."""
+    out = (bits [B,K,W] int32, area [B,K] int32, stability [B,K] fp32, score [B,K] fp32).
+    lengths [B] int32 (device), padded clouds (psam_mask_candidates_varlen_f32): only cloud b's first lengths[b] points are
+    counted and packed, and the slots of its prompts past min(num_prompts, lengths[b]) score -inf."""
     Z, C, N = logits.shape
     bits, area, stab, score = out
     if B < 1 or Z % B or bits.shape[0] != B:
@@ -418,10 +461,18 @@ def mask_candidates_batched(logits: torch.Tensor, iou_preds: torch.Tensor, B: in
         raise ValueError(f"mask_candidates_batched: slots {base}..{base + Zc * C} do not fit {K} candidates per cloud")
     lg = logits.float().contiguous()
     io = iou_preds.float().contiguous()
-    nv.check(nv.lib().psam_mask_candidates_batched_f32(nv.ptr(lg), nv.ptr(io), B, Zc, C, N, float(mask_threshold),
-                                                       float(stability_offset), float(pred_iou_thresh), float(stability_thresh),
-                                                       int(min_area), int(base), K, bits.shape[2], nv.ptr(bits), nv.ptr(area),
-                                                       nv.ptr(stab), nv.ptr(score), nv.stream()), "mask_candidates_batched")
+    if lengths is None:
+        nv.check(nv.lib().psam_mask_candidates_batched_f32(nv.ptr(lg), nv.ptr(io), B, Zc, C, N, float(mask_threshold),
+                                                           float(stability_offset), float(pred_iou_thresh), float(stability_thresh),
+                                                           int(min_area), int(base), K, bits.shape[2], nv.ptr(bits), nv.ptr(area),
+                                                           nv.ptr(stab), nv.ptr(score), nv.stream()), "mask_candidates_batched")
+        return out
+    lengths = _lengths(lengths, B, "mask_candidates_batched")
+    nv.check(nv.lib().psam_mask_candidates_varlen_f32(nv.ptr(lg), nv.ptr(io), nv.ptr(lengths), B, Zc, C, N, int(num_prompts),
+                                                      float(mask_threshold), float(stability_offset), float(pred_iou_thresh),
+                                                      float(stability_thresh), int(min_area), int(base), K, bits.shape[2],
+                                                      nv.ptr(bits), nv.ptr(area), nv.ptr(stab), nv.ptr(score), nv.stream()),
+             "mask_candidates_batched")
     return out
 
 
@@ -441,10 +492,12 @@ def mask_nms_batched(bits: torch.Tensor, area: torch.Tensor, score: torch.Tensor
     return keep, keep_count
 
 
-def mask_regions_batched(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor, nbr: torch.Tensor, min_area: int):
+def mask_regions_batched(bits: torch.Tensor, keep: torch.Tensor, keep_count: torch.Tensor, nbr: torch.Tensor, min_area: int,
+                         lengths: Optional[torch.Tensor] = None):
     """mask_regions on each of B clouds in one launch (psam_mask_regions_batched): candidate masks bits [B,K',W], kept slots
     keep [B,K] with counts keep_count [B], kNN graphs nbr [B,N,k1].  Returns (bits_out [B,K,W], area_out [B,K],
-    score_out [B,K]) by kept rank; nothing waits for the device."""
+    score_out [B,K]) by kept rank; nothing waits for the device.  lengths [B] int32 (device), padded clouds
+    (psam_mask_regions_varlen): cloud b's working sets hold only its first lengths[b] points."""
     B, Kc, W = bits.shape
     K = keep.shape[1]
     N, k1 = nbr.shape[-2], nbr.shape[-1]
@@ -459,9 +512,15 @@ def mask_regions_batched(bits: torch.Tensor, keep: torch.Tensor, keep_count: tor
     area_out = torch.empty((B, K), dtype=torch.int32, device=dev)
     score_out = torch.empty((B, K), dtype=torch.float32, device=dev)
     ws = torch.empty(nv.lib().psam_mask_regions_batched_workspace_bytes(B, K, N), dtype=torch.uint8, device=dev)
-    nv.check(nv.lib().psam_mask_regions_batched(nv.ptr(bits), Kc, B, K, W, N, nv.ptr(keep), nv.ptr(keep_count), nv.ptr(nbr), k1,
-                                                int(min_area), nv.ptr(bits_out), nv.ptr(area_out), nv.ptr(score_out), nv.ptr(ws),
-                                                nv.stream()), "mask_regions_batched")
+    if lengths is None:
+        nv.check(nv.lib().psam_mask_regions_batched(nv.ptr(bits), Kc, B, K, W, N, nv.ptr(keep), nv.ptr(keep_count), nv.ptr(nbr), k1,
+                                                    int(min_area), nv.ptr(bits_out), nv.ptr(area_out), nv.ptr(score_out), nv.ptr(ws),
+                                                    nv.stream()), "mask_regions_batched")
+    else:
+        lengths = _lengths(lengths, B, "mask_regions_batched")
+        nv.check(nv.lib().psam_mask_regions_varlen(nv.ptr(bits), Kc, nv.ptr(lengths), B, K, W, N, nv.ptr(keep), nv.ptr(keep_count),
+                                                   nv.ptr(nbr), k1, int(min_area), nv.ptr(bits_out), nv.ptr(area_out),
+                                                   nv.ptr(score_out), nv.ptr(ws), nv.stream()), "mask_regions_batched")
     return bits_out, area_out, score_out
 
 
