@@ -43,7 +43,9 @@ typedef struct CUstream_st* cudaStream_t;
  * Replaces torkit3d._C.sample_farthest_points_cuda (sample_farthest_points_kernel.cu:106-165, called
  * from pc_sam/model/common.py:91) and batch_index_select (torkit3d/nn/functional.py:34-69, common.py:92).
  * xyz [B,N,3] -> idx_out [B,G] int64 (bit-exact with the reference kernel incl. tie-break),
- * centers_out [B,G,3].  Errors mirror the reference TORCH_CHECKs (:111-115): G<=0 or N<G -> PSAM_ERR_ARG. */
+ * centers_out [B,G,3].  Errors mirror the reference TORCH_CHECKs (:111-115): G<=0 or N<G -> PSAM_ERR_ARG.
+ * workspace: psam_fps_workspace_bytes(B, N, G) bytes; it may be NULL when that is 0, and a NULL workspace where it is not
+ * 0 -> PSAM_ERR_ARG.  Coordinates must be finite: NaN or inf coordinates are outside the contract. */
 size_t psam_fps_workspace_bytes(int B, int N, int G);
 int psam_fps_f32(const float* xyz, int B, int N, int G, long long* idx_out, float* centers_out, void* workspace,
                  cudaStream_t stream);
@@ -59,7 +61,8 @@ int psam_fps_varlen_f32(const float* xyz, const int* lengths, int B, int N_max, 
 /* K nearest keys of every query (exact, direct-difference squared distance, ties by lower index),
  * sorted by (distance, index).  Replaces knn_points = torch.cdist + torch.topk
  * (pc_sam/model/common.py:27-56; call sites :97 and :251).  query [B,Q,3], key [B,N,3] ->
- * idx_out [B,Q,K] int64, d2_out [B,Q,K] squared distances (may be NULL). */
+ * idx_out [B,Q,K] int64, d2_out [B,Q,K] squared distances (may be NULL).  K <= 1024 and B <= 65535, else
+ * PSAM_ERR_UNSUPPORTED.  Coordinates must be finite: NaN or inf coordinates are outside the contract. */
 int psam_knn_f32(const float* query, const float* key, int B, int Q, int N, int K, long long* idx_out, float* d2_out,
                  cudaStream_t stream);
 /* psam_knn_f32 on a padded batch: key [B, N_max, 3], lengths [B]; the keys of cloud b are its first lengths[b] rows, and
@@ -74,7 +77,12 @@ int psam_knn_varlen_f32(const float* query, const float* key, const int* lengths
  * Replaces the fancy-index gathers of KNNGrouper.forward (common.py:99-120) and
  * group_with_centers_and_knn (common.py:126-187).  radius<=0 means None.  feats [B*rep,N,C].
  * center_idx [B,G] (may be NULL) selects centralize_features=True (common.py:116-118, :181-185): C more channels
- * feats[b2,idx] - feats[b2,center_idx[b,g]] are appended (groups_out row = 3 + 2C floats). */
+ * feats[b2,idx] - feats[b2,center_idx[b,g]] are appended (groups_out row = 3 + 2C floats).  N, G, K >= 1.
+ * Rounding, exact: each coordinate is fp32(xyz - centre), times fp32(1 / radius) when radius > 0.  That product is what
+ * torch computes on CUDA for `tensor / radius` with a Python-float radius (a CPU scalar divisor becomes a multiplication
+ * by its fp32 reciprocal, as checked on an H100 with torch 2.11); it differs by 1 ulp from an fp32 division for about
+ * 12 % of uniform values in [-1, 1] at radius 0.05 or 0.1.
+ * Feature channels are copies, and the centralised ones fp32(f - f_centre). */
 int psam_group_gather_f32(const float* xyz, const float* feats, const float* centers, const long long* knn_idx,
                           const long long* center_idx, int B, int rep, int N, int G, int K, int C, float radius,
                           float* groups_out, cudaStream_t stream);
@@ -82,7 +90,13 @@ int psam_group_gather_f32(const float* xyz, const float* feats, const float* cen
 /* Voronoi tokenizer features: out[b2,n,:] = [(xyz[b,n]-c)/max(|xyz[b,n]-c|,1e-8), |xyz[b,n]-c|, feats[b2,n,0:C]] with
  * c = centers[b, nn_idx[b,n]], b = b2/rep.  Replaces NNGrouper.forward / group_with_centers_and_nn
  * (common.py:190-236).  out fp32 [B*rep,N,4+C] and / or the split-bf16 copy y_hi (row pitch `pitch` >= 4+C, zero
- * padded) that feeds PatchEmbedNN.in_proj (pc_encoder.py:186) on the tensor cores. */
+ * padded) that feeds PatchEmbedNN.in_proj (pc_encoder.py:186) on the tensor cores.
+ * Rounding: d = fp32(xyz - c) per axis, dist = sqrtf of the sum of squares, computed as one product and two fused
+ * multiply-adds (three roundings in the sum, halved by the square root, plus the square root's own: relative error at
+ * most 2.5 * 2^-24 against the exact norm of d; 2^-23 would not hold), and
+ * each direction component is the fp32 quotient d / max(dist, 1e-8) - a division, as torch divides by a tensor.  The split
+ * planes are hi = bf16(v), lo = bf16(v - hi) of those fp32 values.  pitch >= 4 + C whenever y_hi is given, and at least
+ * one of out and y_hi, else PSAM_ERR_ARG. */
 int psam_voronoi_features_f32(const float* xyz, const float* centers, const long long* nn_idx, const float* feats, int B,
                               int rep, int N, int G, int C, float* out, void* y_hi, long long y_plane, long long pitch,
                               cudaStream_t stream);
@@ -95,13 +109,16 @@ int psam_scatter_amax_f32(const float* x, const long long* nn_idx, int B, int N,
                           cudaStream_t stream);
 
 /* 3 nearest centres per point and inverse-squared-distance weights.
- * Replaces compute_interp_weights (common.py:238-255).  idx_out [B,N,3] int64, w_out [B,N,3]. */
+ * Replaces compute_interp_weights (common.py:238-255).  idx_out [B,N,3] int64, w_out [B,N,3].  B <= 65535, else
+ * PSAM_ERR_UNSUPPORTED. */
 int psam_knn3_interp_f32(const float* xyz, const float* centers, int B, int N, int G, long long* idx_out, float* w_out,
                          cudaStream_t stream);
 
 /* Nearest-neighbour squared distance (and index) of every query point to a key set; single cloud.
  * Replaces torkit3d chamfer_distance_forward (csrc/cuda/chamfer_distance_kernel.cu:10-151) as used by the
- * ground-truth prompt sampler (pc_sam/model/common.py:447-474): dist1/idx1 only.  idx_out may be NULL. */
+ * ground-truth prompt sampler (pc_sam/model/common.py:447-474): dist1/idx1 only.  idx_out may be NULL.
+ * Ties go to the lower key index.  A key whose squared distance is NaN or not below 3.4e38 (a NaN or inf key) is never
+ * chosen; a query with no such key (a NaN query, for one) gets (3.4e38, -1). */
 int psam_nn_distance_f32(const float* query, const float* key, int n1, int n2, float* dist_out, long long* idx_out,
                          cudaStream_t stream);
 

@@ -329,8 +329,8 @@ __global__ void voronoi_features_kernel(const float* __restrict__ xyz, const flo
         const float* c = centers + ((size_t)b * G + nn_idx[(size_t)b * N + n]) * 3;
         const float dx = p[0] - c[0], dy = p[1] - c[1], dz = p[2] - c[2];
         const float dist = sqrtf(dx * dx + dy * dy + dz * dz);  // torch.linalg.norm: sqrt of the plain sum of squares
-        const float inv = 1.0f / fmaxf(dist, 1e-8f);            // nbr_xyz / clamp(dist, min=1e-8)
-        float v[4] = {dx * inv, dy * inv, dz * inv, dist};
+        const float den = fmaxf(dist, 1e-8f);                   // nbr_xyz / clamp(dist, min=1e-8): a tensor divisor, so
+        float v[4] = {dx / den, dy / den, dz / den, dist};      // torch divides (a reciprocal product is 1 ulp off in ~27 %)
         float* o = out ? out + (size_t)r * CO : nullptr;
         const float* f = feats + (size_t)r * C;
         for (int ch = 0; ch < CO; ++ch) {

@@ -778,6 +778,7 @@ template <bool VARLEN>
 static int knn_dispatch(const float* query, const float* key, const int* lengths, int B, int Q, int N, int K, long long* idx_out,
                         float* d2_out, cudaStream_t stream) {
     if (K > 1024) return PSAM_ERR_UNSUPPORTED;
+    if (B > 65535) return PSAM_ERR_UNSUPPORTED;  // the clouds are the grid's y extent
     const int stride = knn_sample_stride(N, K);
     int sample_cap = (2 * K + 3) & ~3;  // scratch for the final (distance, index) list of one centre
     // candidate capacity per centre: the bound admits ~1.2 K stride keys (sampling std ~ K^-1/2); beyond it the exact fallback runs.
@@ -826,7 +827,8 @@ extern "C" int psam_group_gather_f32(const float* xyz, const float* feats, const
                                      const long long* knn_idx, const long long* center_idx, int B, int rep, int N, int G, int K,
                                      int C, float radius, float* groups_out, cudaStream_t stream) {
     using namespace psam;
-    if (!xyz || !feats || !centers || !knn_idx || !groups_out || B <= 0 || rep <= 0 || C < 0) return PSAM_ERR_ARG;
+    if (!xyz || !feats || !centers || !knn_idx || !groups_out || B <= 0 || rep <= 0 || N <= 0 || G <= 0 || K <= 0 || C < 0)
+        return PSAM_ERR_ARG;
     const long long total = (long long)B * rep * G * K;
     const int blocks = (int)min((long long)132 * 16, ceil_div_ll(total, 256));
     PSAM_CUDA_TRY(psam::launch(group_gather_kernel, dim3(blocks), dim3(256), (size_t)(0), stream, xyz, feats, centers, knn_idx, center_idx, B * rep, rep, N, G, K, C,
@@ -840,7 +842,7 @@ extern "C" int psam_knn3_interp_f32(const float* xyz, const float* centers, int 
     using namespace psam;
     if (!xyz || !centers || !idx_out || !w_out || B <= 0 || N <= 0 || G < 3) return PSAM_ERR_ARG;
     const size_t smem = (size_t)G * 3 * sizeof(float);
-    if (smem > 200 * 1024) return PSAM_ERR_UNSUPPORTED;
+    if (smem > 200 * 1024 || B > 65535) return PSAM_ERR_UNSUPPORTED;  // the clouds are the grid's y extent
     PSAM_CUDA_TRY(cudaFuncSetAttribute(knn3_interp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PSAM_CUDA_TRY(psam::launch(knn3_interp_kernel, dim3(dim3(ceil_div(N, 64), B)), dim3(256), (size_t)(smem), stream, xyz, centers, N, G, idx_out, w_out));
     PSAM_LAUNCH_CHECK();
