@@ -140,6 +140,18 @@ int psam_border_prompt_f32(const float* coords, const unsigned char* gt_masks, c
                            float* prompt_xyz_out, unsigned char* prompt_label_out, int* status, void* workspace,
                            cudaStream_t stream);
 
+/* psam_border_prompt_f32 on a padded batch: coords [B, N_max, 3], lengths [B], gt_masks / pred_logits / pred_masks
+ * [B*M, N_max].  Row i of (cloud b, mask m) takes part only when i < N_b = clamp(lengths[b], 0, N_max): rows at or past
+ * N_b go on neither the foreground nor the background list.  For every (b, m) the prompt xyz and label are bit for bit
+ * those psam_border_prompt_f32 returns on cloud b alone (its first N_b rows of coords, ground truth and prediction), and
+ * *status is set exactly when one of those single-cloud calls would set it (N_b = 0 counts as a mask without a border),
+ * whatever the padding rows hold.  Workspace: psam_border_prompt_workspace_bytes(B, M, N_max).  Refusals: those of
+ * psam_border_prompt_f32, and PSAM_ERR_ARG for a NULL lengths. */
+int psam_border_prompt_varlen_f32(const float* coords, const int* lengths, const unsigned char* gt_masks,
+                                  const float* pred_logits, const unsigned char* pred_masks, int B, int M, int N_max,
+                                  int from_error_region, float* prompt_xyz_out, unsigned char* prompt_label_out, int* status,
+                                  void* workspace, cudaStream_t stream);
+
 /* ---- dense contractions ---------------------------------------------------------------------- */
 
 typedef struct {

@@ -596,6 +596,8 @@ __device__ __forceinline__ int border_region_label(int region, int mode, bool gt
 // Pass 1: compact the foreground AND background point indices of every (cloud x mask, region) - order is irrelevant because
 // min() is order independent and the arg-max key carries the original index.  Warp-aggregated append (one atomic per warp
 // and list); the per-point minimum is initialised to +inf on the way.
+// VARLEN: row i of (cloud x mask) bm takes part only when i < clamp(lengths[bm / M], 0, N) - padded rows go on neither
+// list, so passes 2 and 3 (which read only the lists and counts, and use N as a stride) see exactly the cloud's own rows.
 __device__ __forceinline__ void warp_append(bool pred, int value, int* counter, int* list, unsigned* init_inf) {
     const int lane = threadIdx.x & 31;
     const unsigned m = __ballot_sync(0xffffffffu, pred);
@@ -611,22 +613,25 @@ __device__ __forceinline__ void warp_append(bool pred, int value, int* counter, 
     }
 }
 
+template <bool VARLEN>
 __global__ void __launch_bounds__(256)
 border_compact_kernel(const unsigned char* __restrict__ gt, const float* __restrict__ logits,
-                      const unsigned char* __restrict__ pred_mask, int N, int mode, int nreg, int* __restrict__ counts /* [BM][3][2] */,
-                      int* __restrict__ fg_list, int* __restrict__ bg_list, unsigned* __restrict__ mind /* each [BM][nreg][N] */) {
+                      const unsigned char* __restrict__ pred_mask, const int* __restrict__ lengths, int M, int N, int mode, int nreg,
+                      int* __restrict__ counts /* [BM][3][2] */, int* __restrict__ fg_list, int* __restrict__ bg_list,
+                      unsigned* __restrict__ mind /* each [BM][nreg][N] */) {
     const int bm = blockIdx.y;
     const int i = blockIdx.x * 256 + threadIdx.x;
+    const int n = VARLEN ? min(max(lengths[bm / M], 0), N) : N;
     bool g = false, p = false;
-    if (i < N) {
+    if (i < n) {
         g = gt[(size_t)bm * N + i] != 0;
         p = logits ? (logits[(size_t)bm * N + i] > 0.f) : (pred_mask ? pred_mask[(size_t)bm * N + i] != 0 : false);
     }
     for (int r = 0; r < nreg; ++r) {
         const int lab = border_region_label(r, mode, g, p);
         const size_t off = ((size_t)bm * nreg + r) * N;
-        warp_append(i < N && lab == 1, i, counts + (bm * 3 + r) * 2, fg_list + off, mind + off);
-        warp_append(i < N && lab == 0, i, counts + (bm * 3 + r) * 2 + 1, bg_list + off, nullptr);
+        warp_append(i < n && lab == 1, i, counts + (bm * 3 + r) * 2, fg_list + off, mind + off);
+        warp_append(i < n && lab == 0, i, counts + (bm * 3 + r) * 2 + 1, bg_list + off, nullptr);
     }
 }
 
@@ -731,11 +736,13 @@ extern "C" size_t psam_border_prompt_workspace_bytes(int B, int M, int N) {
     return bm * 6 * 4 + bm * 3 * (size_t)N * 4 * 3;
 }
 
-extern "C" int psam_border_prompt_f32(const float* coords, const unsigned char* gt_masks, const float* pred_logits,
-                                      const unsigned char* pred_masks, int B, int M, int N, int from_error_region,
-                                      float* prompt_xyz_out, unsigned char* prompt_label_out, int* status, void* workspace,
-                                      cudaStream_t stream) {
-    using namespace psam;
+namespace psam {
+
+template <bool VARLEN>
+static int border_prompt_dispatch(const float* coords, const int* lengths, const unsigned char* gt_masks, const float* pred_logits,
+                                  const unsigned char* pred_masks, int B, int M, int N, int from_error_region,
+                                  float* prompt_xyz_out, unsigned char* prompt_label_out, int* status, void* workspace,
+                                  cudaStream_t stream) {
     if (!coords || !gt_masks || !prompt_xyz_out || !prompt_label_out || !status || !workspace || B <= 0 || M <= 0 || N <= 0 ||
         (pred_logits && pred_masks) || ((uintptr_t)workspace & 3) != 0)
         return PSAM_ERR_ARG;
@@ -748,8 +755,8 @@ extern "C" int psam_border_prompt_f32(const float* coords, const unsigned char* 
     int* bg_list = fg_list + (size_t)BM * 3 * N;
     unsigned* mind = reinterpret_cast<unsigned*>(bg_list + (size_t)BM * 3 * N);
     PSAM_CUDA_TRY(cudaMemsetAsync(counts, 0, (size_t)BM * 6 * 4, stream));
-    border_compact_kernel<<<dim3(ceil_div(N, 256), BM), 256, 0, stream>>>(gt_masks, pred_logits, pred_masks, N, mode, nreg, counts, fg_list,
-                                                                         bg_list, mind);
+    border_compact_kernel<VARLEN><<<dim3(ceil_div(N, 256), BM), 256, 0, stream>>>(gt_masks, pred_logits, pred_masks, lengths, M, N, mode,
+                                                                                 nreg, counts, fg_list, bg_list, mind);
     PSAM_LAUNCH_CHECK();
     border_mindist_kernel<<<dim3(ceil_div(N, 512), ceil_div(N, BORDER_CHUNK), BM * nreg), 256, 0, stream>>>(coords, M, N, nreg, counts, fg_list,
                                                                                                           bg_list, mind);
@@ -760,8 +767,24 @@ extern "C" int psam_border_prompt_f32(const float* coords, const unsigned char* 
     return PSAM_OK;
 }
 
-namespace psam {
 }  // namespace psam
+
+extern "C" int psam_border_prompt_f32(const float* coords, const unsigned char* gt_masks, const float* pred_logits,
+                                      const unsigned char* pred_masks, int B, int M, int N, int from_error_region,
+                                      float* prompt_xyz_out, unsigned char* prompt_label_out, int* status, void* workspace,
+                                      cudaStream_t stream) {
+    return psam::border_prompt_dispatch<false>(coords, nullptr, gt_masks, pred_logits, pred_masks, B, M, N, from_error_region,
+                                               prompt_xyz_out, prompt_label_out, status, workspace, stream);
+}
+
+extern "C" int psam_border_prompt_varlen_f32(const float* coords, const int* lengths, const unsigned char* gt_masks,
+                                             const float* pred_logits, const unsigned char* pred_masks, int B, int M, int N_max,
+                                             int from_error_region, float* prompt_xyz_out, unsigned char* prompt_label_out,
+                                             int* status, void* workspace, cudaStream_t stream) {
+    if (!lengths) return PSAM_ERR_ARG;
+    return psam::border_prompt_dispatch<true>(coords, lengths, gt_masks, pred_logits, pred_masks, B, M, N_max, from_error_region,
+                                              prompt_xyz_out, prompt_label_out, status, workspace, stream);
+}
 
 extern "C" int psam_nn_distance_f32(const float* query, const float* key, int n1, int n2, float* dist_out,
                                     long long* idx_out, cudaStream_t stream) {

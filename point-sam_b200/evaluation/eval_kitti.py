@@ -1,7 +1,7 @@
 """Evaluation driver with the behaviour of the reference's evaluation/eval_kitti.py:284-398 on top of the sm_90a
 path: binary PLY crops (fields x y z R G B label) -> normalisation -> per-cloud group-count / group-size override ->
-``model(**data, is_eval=True)`` (iterative GT-driven prompting) -> IoU per prompt iteration, averaged per object class
-and overall.  The dataset glob is an argument instead of a hard-coded path; every crop is rotated by the reference's
+``model.forward_varlen`` on batches of crops of one group shape (``forward(is_eval=True)``'s iterative GT-driven prompting,
+one crop per batch by default) -> IoU per prompt iteration, averaged per object class and overall.  The dataset glob is an argument instead of a hard-coded path; every crop is rotated by the reference's
 fixed R.from_euler("xyz", [-90, 180, 0]) unless --rotation says otherwise (the network is not rotation invariant)."""
 from __future__ import annotations
 
@@ -9,7 +9,7 @@ import argparse
 import glob
 import os
 import sys
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, Hashable, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -17,7 +17,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from pc_sam.model.loss import compute_iou  # noqa: E402
-from pc_sam.utils.ply import normalize_colors, normalize_points, read_ply  # noqa: E402
+from pc_sam.utils.ply import normalize_colors, normalize_points, read_ply, vertex_count  # noqa: E402
 
 
 def transform_fn(x: Dict[str, np.ndarray], device="cuda") -> Dict[str, torch.Tensor]:
@@ -66,23 +66,67 @@ def parse_rotation(spec: Optional[str]) -> Optional[np.ndarray]:
     return euler_xyz_matrix(vals)
 
 
+def group_shape_for(num_points: int) -> Tuple[int, int]:
+    """eval_kitti.py:352-362: the (num_groups, group_size) the reference gives a crop of num_points points."""
+    if num_points > 30000:
+        return 2048, 256
+    return min(num_points, 2048), (2 if num_points < 256 else 256)
+
+
 def set_group_shape(model, num_points: int):
-    """eval_kitti.py:352-362: the tokenizer's group count / size are runtime attributes chosen per cloud.  A hierarchical
+    """The tokenizer's group count / size are runtime attributes chosen per cloud (group_shape_for).  A hierarchical
     tokenizer (PatchEmbedHier: grouper1 / grouper2, which that override does not address) is left as configured."""
     g = getattr(model.pc_encoder.patch_embed, "grouper", None)
     if g is None:
         return
-    if num_points > 30000:
-        g.num_groups, g.group_size = 2048, 256
-    else:
-        g.num_groups, g.group_size = min(num_points, 2048), 256
-        if num_points < 256:
-            g.group_size = 2
+    g.num_groups, g.group_size = group_shape_for(num_points)
+
+
+def plan_eval_batches(sizes: Sequence[int], keys: Sequence[Hashable], batch_size: int,
+                      max_batch_points: int) -> List[List[int]]:
+    """Batches of crop indices for forward_varlen.  Crops are grouped by key (their group shape: crops of different
+    shapes need different G / K and never share a batch), each group is sorted by size so that the padding stays small,
+    and runs of at most batch_size crops with len(batch) * N_max <= max_batch_points are cut from it (a crop larger than
+    the cap runs alone).  The cap bounds the decoder's upscaling input, B * M * N_max * Du * 4 bytes.  Groups come in
+    order of first appearance; every crop appears exactly once."""
+    if batch_size < 1 or max_batch_points < 1:
+        raise ValueError(f"batch_size ({batch_size}) and max_batch_points ({max_batch_points}) must be >= 1")
+    if len(sizes) != len(keys):
+        raise ValueError(f"{len(sizes)} sizes and {len(keys)} keys")
+    groups: Dict[Hashable, List[int]] = {}
+    for i, k in enumerate(keys):
+        groups.setdefault(k, []).append(i)
+    batches: List[List[int]] = []
+    for idx in groups.values():
+        cur: List[int] = []
+        for i in sorted(idx, key=lambda j: (sizes[j], j)):
+            if cur and (len(cur) + 1 > batch_size or (len(cur) + 1) * sizes[i] > max_batch_points):
+                batches.append(cur)
+                cur = []
+            cur.append(i)
+        batches.append(cur)
+    return batches
+
+
+def _run_batch(model, data: List[Dict[str, torch.Tensor]]):
+    """One batch of transformed crops -> forward_varlen's per-crop lists.  A model with only the reference's forward (no
+    forward_varlen) is run on a batch of one crop through forward, whose outputs have the same structure for B = 1."""
+    if hasattr(model, "forward_varlen"):
+        return model.forward_varlen([d["coords"][0] for d in data], [d["features"][0] for d in data],
+                                    [d["gt_masks"][0] for d in data], is_eval=True)
+    if len(data) != 1:
+        raise TypeError(f"{type(model).__name__} has no forward_varlen: evaluate it with batch_size=1")
+    return [model(**data[0], is_eval=True)]
 
 
 def evaluate(model, files: Sequence[str], rotation: Optional[np.ndarray] = None, log=print, rank: Optional[int] = None,
-             world: Optional[int] = None) -> Dict[str, object]:
+             world: Optional[int] = None, batch_size: int = 1, max_batch_points: int = 1 << 20) -> Dict[str, object]:
     """Returns {"total": [prompt_iters], "per_object": {name: [prompt_iters]}, "object_mean": [prompt_iters]}.
+
+    Crops run in batches of up to batch_size through model.forward_varlen (batch size 1 included, so there is one code
+    path): plan_eval_batches groups them by group shape and size from their PLY headers, and each batch's crops are read
+    only when it runs.  A crop whose labels are all 0 or all 1 has no border to sample prompts from and is refused
+    (RuntimeError naming it).  IoU rows are kept in file order.
 
     Crops are independent, so with several processes (one per GPU, torch.distributed initialised) each rank evaluates a
     contiguous slice of `files` and the per-crop IoU rows are all-gathered once at the end; every rank
@@ -96,18 +140,31 @@ def evaluate(model, files: Sequence[str], rotation: Optional[np.ndarray] = None,
         world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         rank = dist.get_rank() if world > 1 else 0
     lo, hi = shard_range(len(files), rank or 0, world)
-    rows: List[np.ndarray] = []
+    mine = files[lo:hi]
+    sizes = [vertex_count(p) for p in mine]
+    flat = getattr(model.pc_encoder.patch_embed, "grouper", None) is not None
+    keys = [group_shape_for(n) if flat else None for n in sizes]  # a hierarchical tokenizer keeps one shape
+    rows: List[Optional[np.ndarray]] = [None] * len(mine)
     model.eval()
     dev = next(model.parameters()).device
     with torch.no_grad():
-        for path in files[lo:hi]:
-            data = transform_fn(load_crop(path, rotation), device=dev)
-            set_group_shape(model, data["coords"].shape[1])
-            outputs = model(**data, is_eval=True)
-            gt = data["gt_masks"].flatten(0, 1)
-            rows.append(np.array([compute_iou(o["prompt_masks"], gt).detach().cpu().numpy().mean() for o in outputs]))
+        for batch in plan_eval_batches(sizes, keys, batch_size, max_batch_points):
+            data = []
+            for i in batch:
+                crop = load_crop(mine[i], rotation)
+                fg = crop["mask"] != 0
+                if not fg.any() or fg.all():
+                    raise RuntimeError(f"{mine[i]}: every label is {int(fg[0])}, so the ground truth has no border to "
+                                       "sample prompts from")
+                data.append(transform_fn(crop, device=dev))
+            set_group_shape(model, sizes[batch[0]])  # one key per batch
+            outs = _run_batch(model, data)
+            ious = torch.stack([torch.stack([compute_iou(o["prompt_masks"], d["gt_masks"][0]) for o in out])
+                                for out, d in zip(outs, data)])  # [len(batch), prompt_iters, M]
+            for i, r in zip(batch, ious.cpu().numpy()):  # one host copy per batch
+                rows[i] = r.mean(axis=-1)
             if log:
-                log(f"[rank {rank or 0}] current mean IoU: {np.array(rows).mean(axis=0)}")
+                log(f"[rank {rank or 0}] current mean IoU: {np.array([r for r in rows if r is not None]).mean(axis=0)}")
     iters = int(getattr(model, "prompt_iters", rows[0].shape[0] if rows else 0))
     local = torch.tensor(np.array(rows), dtype=torch.float32).reshape(len(rows), iters)
     if world > 1:
@@ -135,6 +192,10 @@ def main(argv=None):
     ap.add_argument("--data", type=str, required=True, help="glob of binary PLY crops (x y z R G B label)")
     ap.add_argument("--rotation", type=str, default="reference",
                     help="'reference' = euler xyz -90,180,0 deg as eval_kitti.py:18 (default), 'none', or 'ax,ay,az' in degrees")
+    ap.add_argument("--batch-size", type=int, default=1,
+                    help="crops of the same group shape evaluated together in one padded batch (forward_varlen)")
+    ap.add_argument("--max-batch-points", type=int, default=1 << 20,
+                    help="cap on crops x largest crop size per batch (bounds the decoder's memory)")
     args, overrides = ap.parse_known_args(argv)
     cfg = compose(args.config_dir, args.config, overrides)["model"] if args.config_dir else model_config(args.config)
     torch.manual_seed(42)
@@ -149,7 +210,8 @@ def main(argv=None):
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
     model.eval().cuda()
-    res = evaluate(model, sorted(glob.glob(args.data)), rotation=parse_rotation(args.rotation))
+    res = evaluate(model, sorted(glob.glob(args.data)), rotation=parse_rotation(args.rotation), batch_size=args.batch_size,
+                   max_batch_points=args.max_batch_points)
     if int(os.environ.get("RANK", "0")) == 0:
         print(f"Total mean IoU: {res['total']}")
         print(f"Object mean IoU: {res['object_mean']}")

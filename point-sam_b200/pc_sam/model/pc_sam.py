@@ -71,7 +71,7 @@ class PointCloudSAM(nn.Module):
         """Checks a batch of clouds of different sizes without touching the device and returns their sizes N_b: coords and
         features are sequences of B >= 1 tensors [N_b, 3] and [N_b, Cf].  A Voronoi tokenizer (PatchEmbedNN) is refused
         (NotImplementedError: padded points would join its cells' maxima), and so is a cloud smaller than the first-level
-        num_groups (RuntimeError, as for one cloud)."""
+        num_groups or group_size (RuntimeError, as for one cloud: its kNN groups would take padded rows as neighbours)."""
         if isinstance(self.pc_encoder.patch_embed, PatchEmbedNN):
             raise NotImplementedError("clouds of different sizes need a kNN tokenizer: the Voronoi tokenizer (PatchEmbedNN) "
                                       "would pool padded points into its cells")
@@ -85,9 +85,64 @@ class PointCloudSAM(nn.Module):
             if c.dim() != 2 or c.shape[1] != 3 or f.dim() != 2 or f.shape[0] != c.shape[0]:
                 raise ValueError(f"cloud {b}: coords {tuple(c.shape)} and features {tuple(f.shape)} must be [N_b, 3] and [N_b, C]")
             sizes.append(int(c.shape[0]))
-        if min(sizes) < self._group_shape()[0]:
+        num_groups, group_size = self._group_shape()[:2]
+        if min(sizes) < num_groups:
             raise RuntimeError("sample_farthest_points: number of points must be >= num_samples")
+        if min(sizes) < group_size:
+            b = sizes.index(min(sizes))
+            raise RuntimeError(f"knn: cloud {b} has {sizes[b]} points, fewer than the group size {group_size} (k nearest "
+                               "neighbours need k <= number of points)")
         return sizes
+
+    def _varlen_gt(self, gt_masks: Sequence[torch.Tensor], sizes: List[int]) -> List[torch.Tensor]:
+        """Checks per-cloud ground truth against the cloud sizes without touching the device: gt_masks is a sequence of
+        [M, N_b] or [N_b] tensors with the same M for every cloud.  Returns them as [M, N_b]."""
+        if torch.is_tensor(gt_masks):
+            raise TypeError("gt_masks must be a sequence of [M, N_b] / [N_b] tensors, one per cloud")
+        gts = [g.unsqueeze(0) if g.dim() == 1 else g for g in gt_masks]
+        if len(gts) != len(sizes):
+            raise ValueError(f"{len(gts)} ground-truth tensors for {len(sizes)} clouds")
+        for b, (g, n) in enumerate(zip(gts, sizes)):
+            if g.dim() != 2 or g.shape[1] != n or g.shape[0] != gts[0].shape[0] or g.shape[0] < 1:
+                raise ValueError(f"cloud {b}: ground truth {tuple(gt_masks[b].shape)} must be [M, {n}] or [{n}], with the "
+                                 f"same M >= 1 for every cloud (cloud 0 has M = {gts[0].shape[0]})")
+        return gts
+
+    def forward_varlen(self, coords: Sequence[torch.Tensor], features: Sequence[torch.Tensor],
+                       gt_masks: Sequence[torch.Tensor], is_eval: bool = True) -> List[List[Dict[str, torch.Tensor]]]:
+        """forward(is_eval=True) on B clouds of different sizes with one encode: coords / features / gt_masks are sequences
+        of [N_b, 3], [N_b, C] and [M, N_b] or [N_b] bool tensors (the same M for every cloud).  The clouds are padded to
+        N_max = max N_b (ops.pad_clouds) and run through the same `prompt_iters` rounds as forward, with the same host
+        checks per round; FPS, kNN and the ground-truth prompt sampler stay inside each cloud, and the decoder also computes
+        the padded rows, which are dropped.  Returns B lists; list b has forward's structure for cloud b alone (masks
+        [M, C, N_b], prompt_masks [M, N_b], prompt_coords [M, t + 1, 3], ...) as views of the batch outputs.
+        Refused before any device work: training mode or is_eval=False (NotImplementedError: the random training sampler
+        is not length-aware), the Voronoi tokenizer and clouds below the first-level group shape (varlen_clouds), and
+        shape mismatches (ValueError)."""
+        if self.training or not is_eval:
+            raise NotImplementedError("forward_varlen runs the evaluation loop only: call model.eval() and pass is_eval=True "
+                                      "(the random training sampler does not take clouds of different sizes)")
+        sizes = self.varlen_clouds(coords, features)
+        gts = self._varlen_gt(gt_masks, sizes)
+        B, M = len(sizes), gts[0].shape[0]
+        xyz, rgb, lengths = ops.pad_clouds(coords, features)
+        gt = torch.zeros((B, M, xyz.shape[1]), dtype=torch.bool, device=xyz.device)
+        for b, (g, n) in enumerate(zip(gts, sizes)):
+            gt[b, :, :n].copy_(g, non_blocking=True)
+        enc = self._encode(xyz, rgb, lengths)
+        return self._split_varlen(self._eval_loop(enc, xyz, gt, is_eval=True, lengths=lengths), sizes, M)
+
+    @staticmethod
+    def _split_varlen(outputs, sizes: List[int], M: int) -> List[List[Dict[str, torch.Tensor]]]:
+        """Per-iteration dicts of a padded batch -> one list per cloud, each field a view cut to cloud b."""
+        per = []
+        for b, n in enumerate(sizes):
+            s = slice(b * M, (b + 1) * M)
+            per.append([dict(prompt_coords=o["prompt_coords"][s], prompt_labels=o["prompt_labels"][s],
+                             masks=o["masks"][s, :, :n], iou_preds=o["iou_preds"][s],
+                             max_iou_pred_ind=o["max_iou_pred_ind"][s] if torch.is_tensor(o["max_iou_pred_ind"]) else o["max_iou_pred_ind"],
+                             prompt_masks=o["prompt_masks"][s, :n]) for o in outputs])
+        return per
 
     def predict_masks_varlen(self, coords: Sequence[torch.Tensor], features: Sequence[torch.Tensor], prompt_coords: torch.Tensor,
                              prompt_labels: torch.Tensor, prompt_masks: Optional[Sequence[torch.Tensor]] = None,
@@ -117,10 +172,10 @@ class PointCloudSAM(nn.Module):
                                   bool(multimask_output))
         return [(masks[b * M:(b + 1) * M, :, :n], iou[b * M:(b + 1) * M]) for b, n in enumerate(sizes)]
 
-    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval):
+    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval, lengths=None):
         from .prompt_sampling import sample_prompts_adapter
 
-        return sample_prompts_adapter(coords, gt_masks, prompt_masks, is_eval=is_eval)
+        return sample_prompts_adapter(coords, gt_masks, prompt_masks, is_eval=is_eval, lengths=lengths)
 
     # ------------------------------------------------------------------------------------------
     def set_pointcloud(self, xyz: torch.Tensor, rgb: torch.Tensor):
@@ -181,6 +236,15 @@ class PointCloudSAM(nn.Module):
 
         return IterativeGraphPredictor(self, batch_size, num_masks, num_points, use_graph, throughput_tiles=throughput_tiles)
 
+    def make_iterative_predictor_varlen(self, batch_size: int, num_masks: int, max_points: int, use_graph: bool = True,
+                                        throughput_tiles: bool = False):
+        """forward_varlen as ONE CUDA graph for every batch of up to batch_size clouds of at most max_points points each
+        with num_masks ground-truth masks: the lengths live in a device buffer that FPS, kNN and the prompt sampler read,
+        so no cloud size is baked into the graph.  Returns forward_varlen's structure (views valid until the next call)."""
+        from psam_b200.predictor import IterativeGraphPredictorVarlen
+
+        return IterativeGraphPredictorVarlen(self, batch_size, num_masks, max_points, use_graph, throughput_tiles=throughput_tiles)
+
     # ------------------------------------------------------------------------------------------
     def predict_iterative(self, coords, features, prompt_coords_seq: List[torch.Tensor],
                           prompt_labels_seq: List[torch.Tensor]) -> List[Dict[str, torch.Tensor]]:
@@ -218,14 +282,19 @@ class PointCloudSAM(nn.Module):
         if gt_masks.dim() == 2:
             gt_masks = gt_masks.unsqueeze(1)
         gt_masks = gt_masks.bool()
-        B, M = coords.shape[0], gt_masks.shape[1]
         enc = self._encode(coords.float().contiguous(), features.float().contiguous())
+        return self._eval_loop(enc, coords, gt_masks, is_eval)
+
+    def _eval_loop(self, enc, coords, gt_masks, is_eval, lengths=None):
+        """The body of forward after the encode: `prompt_iters` rounds of prompt sampling from the ground truth
+        gt_masks [B, M, N] bool, decode and best-mask feedback.  lengths: padded clouds (forward_varlen)."""
+        B, M = coords.shape[0], gt_masks.shape[1]
         outputs = []
         pc = coords.new_empty((B * M, 0, 3))
         pl = gt_masks.new_empty((B * M, 0))
         pm = None
         for i in range(self.prompt_iters):
-            npc, npl = self._sample_prompts(coords, gt_masks, pm, is_eval)
+            npc, npl = self._sample_prompts(coords, gt_masks, pm, is_eval, lengths)
             pc = torch.cat([pc, npc], dim=1)
             pl = torch.cat([pl, npl], dim=1)
             masks, iou = self._decode(enc, pc, pl, pm, i == 0, center_idx=self._center_idx(enc))
@@ -279,9 +348,9 @@ class PointCloudSAMHier(PointCloudSAM):
         pe = self.pc_encoder.patch_embed
         return pe.grouper1.num_groups, pe.grouper1.group_size, pe.grouper2.num_groups, pe.grouper2.group_size
 
-    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval):
-        if is_eval:
-            return super()._sample_prompts(coords, gt_masks, prompt_masks, is_eval)
+    def _sample_prompts(self, coords, gt_masks, prompt_masks, is_eval, lengths=None):
+        if is_eval or lengths is not None:
+            return super()._sample_prompts(coords, gt_masks, prompt_masks, is_eval, lengths)
         from .prompt_sampling import sample_prompts
 
         return sample_prompts(coords, gt_masks, prompt_masks)

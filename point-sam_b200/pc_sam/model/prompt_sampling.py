@@ -27,8 +27,9 @@ def sample_furthest_points_from_border(coords: torch.Tensor, labels: torch.Tenso
 
 
 @torch.no_grad()
-def sample_fixed_points(points, gt_masks, pred_logits, threshold=None, from_error_region=False):
-    """points [B,N,3], gt_masks [B,M,N] bool, pred_logits [B*M,N] | None -> ([B*M,1,3], [B*M,1] bool)."""
+def sample_fixed_points(points, gt_masks, pred_logits, threshold=None, from_error_region=False, *, lengths=None):
+    """points [B,N,3], gt_masks [B,M,N] bool, pred_logits [B*M,N] | None -> ([B*M,1,3], [B*M,1] bool).
+    lengths [B] int32 (device): padded clouds (ops.pad_clouds); each cloud samples among its first lengths[b] rows only."""
     B, M, N = gt_masks.shape
     logits = masks = None
     if pred_logits is not None:
@@ -38,7 +39,7 @@ def sample_fixed_points(points, gt_masks, pred_logits, threshold=None, from_erro
         else:
             masks = pred_logits.sigmoid() > threshold
     xyz, labels, _ = ops.border_prompt(points, gt_masks.bool(), logits, masks, from_error_region,
-                                       status=engine.sampler_flag(points.device))
+                                       status=engine.sampler_flag(points.device), lengths=lengths)
     engine.raise_if_sampler_failed(points.device)  # the one host check per prompt iteration (skipped under graph capture)
     return xyz, labels
 
@@ -65,9 +66,16 @@ def sample_prompts(points, gt_masks, pred_logits, threshold=None):
 
 
 @torch.no_grad()
-def sample_prompts_adapter(points, gt_masks, pred_logits: Union[torch.Tensor, None], threshold=None, is_eval=False):
+def sample_prompts_adapter(points, gt_masks, pred_logits: Union[torch.Tensor, None], threshold=None, is_eval=False, *,
+                           lengths=None):
     """common.py:287-318: first iteration samples inside the ground truth, later ones inside the error regions; the
-    random sampler is only used in training once the batch IoU has reached 1."""
+    random sampler is only used in training once the batch IoU has reached 1.  lengths: padded clouds, evaluation only
+    (NotImplementedError with is_eval=False: the random training sampler does not take lengths)."""
+    if lengths is not None:
+        if not is_eval:
+            raise NotImplementedError("prompt sampling on padded clouds (lengths) is implemented for is_eval=True only")
+        return sample_fixed_points(points, gt_masks, pred_logits, threshold, from_error_region=pred_logits is None,
+                                   lengths=lengths)
     if pred_logits is None:
         return sample_fixed_points(points, gt_masks, pred_logits, threshold, from_error_region=True)
     if not is_eval:

@@ -110,6 +110,17 @@ def read_ply(filename, triangular_mesh: bool = False, allow_ascii: bool = False)
         return [data, faces]
 
 
+def vertex_count(filename) -> int:
+    """Number of vertices from the header alone (the payload is not read): the ``vertex`` element's count, or the first
+    element's as read_ply uses it."""
+    with open(filename, "rb") as f:
+        h = parse_header(f)
+    v = h.element("vertex") or (h.elements[0] if h.elements else None)
+    if v is None:
+        raise ValueError("PLY file without elements")
+    return v[1]
+
+
 def write_ply(filename, fields: Dict[str, np.ndarray], fmt: str = "binary_little_endian"):
     """Writer used by the tests and by ``save`` of the demo session: one scalar property per dict entry."""
     names = list(fields)

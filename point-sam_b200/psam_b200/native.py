@@ -58,7 +58,7 @@ class LnArgs(Structure):
 EXPORTS = [
     "psam_fps_workspace_bytes", "psam_fps_f32", "psam_knn_f32", "psam_group_gather_f32", "psam_knn3_interp_f32", "psam_nn_distance_f32",
     "psam_voronoi_features_f32", "psam_scatter_amax_f32",
-    "psam_border_prompt_workspace_bytes", "psam_border_prompt_f32",
+    "psam_border_prompt_workspace_bytes", "psam_border_prompt_f32", "psam_border_prompt_varlen_f32",
     "psam_gemm_bf16x3", "psam_gemm_rowln_bf16x3", "psam_attention_bf16x3", "psam_attention_bf16x3_twopass", "psam_linear_f32", "psam_layernorm_f32", "psam_swiglu_ln", "psam_small_in_linear",
     "psam_group_max", "psam_softmax_split", "psam_transpose_split", "psam_posenc_f32", "psam_attention_f32",
     "psam_decoder_prepare", "psam_interp_ln_gelu", "psam_interp_add_ln_gelu", "psam_mask_dot", "psam_add_bcast_f32", "psam_split_f32", "psam_split_add_f32",
@@ -114,6 +114,7 @@ def lib():
             "psam_knn3_interp_f32": [p, p, i, i, i, p, p, p],
             "psam_nn_distance_f32": [p, p, i, i, p, p, p],
             "psam_border_prompt_f32": [p, p, p, p, i, i, i, i, p, p, p, p, p],
+            "psam_border_prompt_varlen_f32": [p, p, p, p, p, i, i, i, i, p, p, p, p, p],
             "psam_gemm_bf16x3": [POINTER(Operand), POINTER(Operand), POINTER(GemmOut), i, i, p],
             "psam_gemm_rowln_bf16x3": [POINTER(Operand), POINTER(Operand), p, ll, i, p, p, f, i, p, ll, ll, i, p],
             "psam_attention_bf16x3": [POINTER(Operand), POINTER(Operand), POINTER(Operand), p, ll, ll, ll, ll, f, p],

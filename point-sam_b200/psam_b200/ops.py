@@ -175,10 +175,14 @@ def nn_distance(query: torch.Tensor, key: torch.Tensor):
 
 def border_prompt(coords: torch.Tensor, gt_masks: torch.Tensor, pred_logits: Optional[torch.Tensor] = None,
                   pred_masks: Optional[torch.Tensor] = None, from_error_region: bool = False,
-                  status: Optional[torch.Tensor] = None):
+                  status: Optional[torch.Tensor] = None, lengths: Optional[torch.Tensor] = None):
     """Batched farthest-from-border prompt sampling (psam_border_prompt_f32).  coords [B,N,3], gt_masks [B,M,N] bool,
-    prediction as logits [B*M,N] or bool masks [B*M,N] or neither.  Returns (xyz [B*M,1,3], labels [B*M,1] bool, status)."""
+    prediction as logits [B*M,N] or bool masks [B*M,N] or neither.  Returns (xyz [B*M,1,3], labels [B*M,1] bool, status).
+    lengths [B] int32 (device): padded clouds, cloud b is its first lengths[b] rows (psam_border_prompt_varlen_f32); each
+    (cloud, mask) gets what the single-cloud sampler returns on that cloud alone."""
     B, M, N = gt_masks.shape
+    if lengths is not None:
+        lengths = _lengths(lengths, B, "border_prompt")
     c = coords.float().contiguous()
     g = gt_masks.contiguous().view(torch.uint8) if gt_masks.dtype == torch.bool else gt_masks.to(torch.uint8).contiguous()
     lg = pred_logits.float().contiguous() if pred_logits is not None else None
@@ -191,8 +195,13 @@ def border_prompt(coords: torch.Tensor, gt_masks: torch.Tensor, pred_logits: Opt
     if status is None:
         status = torch.zeros(1, dtype=torch.int32, device=dev)
     ws = torch.empty(nv.lib().psam_border_prompt_workspace_bytes(B, M, N), dtype=torch.uint8, device=dev)
-    nv.check(nv.lib().psam_border_prompt_f32(nv.ptr(c), nv.ptr(g), nv.ptr(lg), nv.ptr(pm), B, M, N, int(from_error_region), nv.ptr(xyz),
-                                             nv.ptr(lab), nv.ptr(status), nv.ptr(ws), nv.stream()), "border_prompt")
+    if lengths is None:
+        nv.check(nv.lib().psam_border_prompt_f32(nv.ptr(c), nv.ptr(g), nv.ptr(lg), nv.ptr(pm), B, M, N, int(from_error_region),
+                                                 nv.ptr(xyz), nv.ptr(lab), nv.ptr(status), nv.ptr(ws), nv.stream()), "border_prompt")
+    else:
+        nv.check(nv.lib().psam_border_prompt_varlen_f32(nv.ptr(c), nv.ptr(lengths), nv.ptr(g), nv.ptr(lg), nv.ptr(pm), B, M, N,
+                                                        int(from_error_region), nv.ptr(xyz), nv.ptr(lab), nv.ptr(status), nv.ptr(ws),
+                                                        nv.stream()), "border_prompt")
     return xyz, lab.view(torch.bool), status
 
 

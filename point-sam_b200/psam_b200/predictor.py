@@ -179,6 +179,66 @@ class IterativeGraphPredictor:
             engine.raise_if_sampler_failed(self.dev)
 
 
+class IterativeGraphPredictorVarlen(IterativeGraphPredictor):
+    """PointCloudSAM.forward_varlen as one CUDA graph: static padded buffers xyz / feats [B, N_max, 3], gt [B, M, N_max]
+    and lengths [B] (int32, device).  FPS's tie-break block size, the kNN bound and the prompt sampler read the lengths on
+    the device, so one capture serves every batch of up to B clouds of at most N_max points each.  Inputs are sequences of
+    [N_b, 3], [N_b, 3] and [M, N_b] or [N_b] tensors, as for forward_varlen; the call returns forward_varlen's per-cloud
+    lists as views of the graph's outputs, valid until the next call."""
+
+    def __init__(self, model, B: int, M: int, N_max: int, use_graph: bool = True, device=None, throughput_tiles: bool = False):
+        super().__init__(model, B, M, N_max, use_graph, device, throughput_tiles)
+        self.lengths = torch.zeros(B, dtype=torch.int32, device=self.dev)
+        self.sizes = []
+
+    def _run(self):
+        with engine.flag_scope(range_flag=self.flag, sampler=self.sflag):
+            enc = self.model._encode(self.xyz, self.feats, self.lengths)
+            return self.model._eval_loop(enc, self.xyz, self.gt, True, self.lengths)
+
+    def _check(self, coords, features, gt_masks):
+        """Host-side refusals, before anything is enqueued."""
+        B, M, N_max = self.gt.shape
+        if torch.is_tensor(coords) or torch.is_tensor(features):
+            raise TypeError("coords and features must be sequences of [N_b, 3] tensors, one per cloud")
+        coords, features = list(coords), list(features)
+        if len(coords) > B:
+            raise ValueError(f"{len(coords)} clouds for a predictor of at most {B}")
+        sizes = self.model.varlen_clouds(coords, features)
+        if max(sizes) > N_max:
+            raise ValueError(f"cloud {sizes.index(max(sizes))} has {max(sizes)} points, more than the predictor's {N_max}")
+        if any(f.shape[1] != self.feats.shape[2] for f in features):
+            raise ValueError(f"features must be [N_b, {self.feats.shape[2]}]")
+        gts = self.model._varlen_gt(gt_masks, sizes)
+        if gts[0].shape[0] != M:
+            raise ValueError(f"ground truth has {gts[0].shape[0]} masks per cloud, the predictor {M}")
+        return coords, features, gts, sizes
+
+    def _load(self, coords, features, gt_masks, caller=None):
+        """Cloud b goes to rows 0 .. N_b - 1 of slot b and the rest of the slot is zeroed; slots past the given clouds get
+        a copy of the last one (a zero-length cloud would have no border to sample), and their outputs are not returned."""
+        coords, features, gts, sizes = self._check(coords, features, gt_masks)
+        if caller is not None and caller != self.stream and any(t.is_cuda for t in (*coords, *features, *gts)):
+            self.stream.wait_stream(caller)
+        slots = [min(b, len(sizes) - 1) for b in range(self.gt.shape[0])]
+        self.xyz.zero_()
+        self.feats.zero_()
+        self.gt.zero_()
+        for b, s in enumerate(slots):
+            n = sizes[s]
+            self.xyz[b, :n].copy_(coords[s], non_blocking=True)
+            self.feats[b, :n].copy_(features[s], non_blocking=True)
+            self.gt[b, :, :n].copy_(gts[s], non_blocking=True)
+        # a fresh pinned tensor per call: a copy still pending from the previous call is never overwritten
+        host = torch.tensor([sizes[s] for s in slots], dtype=torch.int32).pin_memory()
+        self.lengths.copy_(host, non_blocking=True)
+        self.sizes = sizes
+
+    def __call__(self, coords, features, gt_masks, check: bool = True):
+        outputs = super().__call__(coords, features, gt_masks, check)
+        return self.model._split_varlen(outputs, self.sizes, self.gt.shape[1])
+
+
 class PipelinedPredictor:
     """Serving front-end: `depth` independent GraphPredictors (own stream, own CUDA graph, own static buffers,
     shared weights) used round-robin, so consecutive clouds overlap on the GPU - cloud i+1's latency-bound FPS /
