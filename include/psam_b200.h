@@ -536,6 +536,61 @@ int psam_crop_uncrop(const uint32_t* bits, const int* area, const float* score, 
                      uint32_t* gbits, int* garea, float* giou, float* gstab, long long* gprompt, int* gslot, int* gcrop,
                      float* gscore, int* overflow, cudaStream_t stream);
 
+/* Crop layers on a batch of B clouds.  Each entry point below gives every cloud (or crop) the result of its single-cloud
+ * counterpart above bit for bit; the single-cloud entry points are the case B = 1 of the same kernels.
+ *
+ * Batched layout: psam_crop_layout_f32 on each cloud of xyz [B, N_max, 3]: boxes [B, T, 6] and counts [B, T] with
+ * T = psam_crop_total(n_layers).  lengths [B] (device int32, NULL: every cloud has N_max points): cloud b is its first
+ * clamp(lengths[b], 0, N_max) rows; the rows past it are never read, so they touch neither its bounding box nor any count
+ * whatever they hold (NaN included).  1 <= B <= 65535.  Two launches.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_crop_layout_batched_f32(const float* xyz, const int* lengths, int B, int N_max, int n_layers, float overlap_ratio,
+                                 float* boxes, int* counts, cudaStream_t stream);
+/* Batched gather: P (cloud, crop) pairs of the batched layout into one padded batch of crop clouds.  pairs [3, P] (device
+ * int32): row 0 the clouds (0 .. B-1), row 1 the crops (0 .. n_crops-1), row 2 the counts (the layout's count of that crop,
+ * 0 .. n_max).  xyz / rgb [B, N_max, 3] and lengths as for the layout; boxes [B, n_crops, 6].  Outputs: idx_out [P, n_max],
+ * xyz_out / rgb_out [P, n_max, 3] and edge [P, ceil(n_max / 32)]; row p's first counts[p] entries equal
+ * psam_crop_gather_f32(cloud's points, crop, n_out = counts[p]) bit for bit (same stable compaction, the edge margin from
+ * the cloud's own bounding box), its later rows are 0 and its edge bits past counts[p] are 0.  A pair outside these ranges
+ * gathers nothing (all its rows 0).  1 <= P <= 65535, 1 <= n_max <= N_max.  Two launches.  workspace:
+ * psam_crop_gather_batched_workspace_bytes(P, N_max) bytes, 16-byte aligned.  Bad arguments -> PSAM_ERR_ARG before any CUDA
+ * call. */
+size_t psam_crop_gather_batched_workspace_bytes(int P, int N_max);
+int psam_crop_gather_batched_f32(const float* xyz, const float* rgb, const int* lengths, int B, int N_max, const float* boxes,
+                                 int n_crops, const int* pairs, int P, int n_max, float edge_margin, int* idx_out, float* xyz_out,
+                                 float* rgb_out, uint32_t* edge, void* workspace, cudaStream_t stream);
+/* Batched edge filter: psam_crop_edge_filter on each crop t < T of bits [T, K, W], edge [T, W] and score [T, K], one launch.
+ * 1 <= T <= 65535; bits / edge / score may be NULL when K == 0.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_crop_edge_filter_batched(const uint32_t* bits, int T, int K, int W, const uint32_t* edge, float* score,
+                                  cudaStream_t stream);
+/* Batched uncrop: psam_crop_uncrop for R crop runs of B clouds in one launch.  runs[R] (device memory) describes each run
+ * with the arguments of psam_crop_uncrop (its candidates, keep list of K entries, kept count, crop point indices idx of its
+ * n points, prompt indices, slots, crop number and layer score), its cloud, and the cloud's capacity (<= cloud_rows).
+ * The runs of one cloud are consecutive and in that cloud's crop order; `first` is the index of its cloud's first run and
+ * `last` is 1 for its cloud's last run.  Run r's masks go to cloud c's rows of gbits [B, cloud_rows, Wg] and of the per-mask
+ * outputs [B, cloud_rows], starting at the exclusive prefix (in run order) of the kept counts of the cloud's earlier runs,
+ * computed on the device: the result equals psam_crop_uncrop over the cloud's runs in order.  The cloud's last run writes
+ * lifted[c] (the total kept count) and overflow[c] (1 when that exceeds the capacity, else 0); no other CTA writes them.
+ * Every cloud needs at least one run.  1 <= R <= 65535, K_max >= every run's K, Wg >= ceil(N_max / 32) with every run's
+ * idx < N_max, 1 <= cloud_rows <= 16384.  Bad arguments -> PSAM_ERR_ARG before any CUDA call.
+ * psam_crop_run_bytes() = sizeof(psam_crop_run), for bindings that lay the table out themselves. */
+typedef struct psam_crop_run {
+    const uint32_t* bits;           /* [K', W] candidates */
+    const int* area;
+    const float* score;
+    const float* stability;
+    const int* keep;                /* [K] kept slots */
+    const int* keep_count;          /* [1] */
+    const int* idx;                 /* [n] the crop's point indices in its cloud */
+    const long long* prompt_index;  /* crop-local prompt indices */
+    int K, W, n, slots, crop, cloud, first, last;
+    float layer_score;
+    int capacity;
+} psam_crop_run;
+size_t psam_crop_run_bytes(void);
+int psam_crop_uncrop_batched(const psam_crop_run* runs, int R, int K_max, int B, int N_max, int Wg, int cloud_rows, uint32_t* gbits,
+                             int* garea, float* giou, float* gstab, long long* gprompt, int* gslot, int* gcrop, float* gscore,
+                             int* lifted, int* overflow, cudaStream_t stream);
+
 /* ---- meshes and dense clouds ---------------------------------------------------------------------- */
 /* Area-weighted surface sampling of a triangle mesh: vertices [V, 3] fp32, faces [F, 3] int32 -> S samples xyz_out [S, 3],
  * rgb_out [S, 3] and face_out [S] (int32, the face each sample lies on).  Everything is fp32, every operation rounded on its

@@ -12,6 +12,10 @@
 //   crop_edge_filter_kernel   one warp per candidate: any(bits & edge) -> score = -inf.
 //   crop_uncrop_kernel        persistent CTAs over the kept ranks: zero the global row, scatter the local bits through the
 //                             crop's index list, copy the per-mask fields; appends at a device-side offset.
+//
+// Batches of clouds: every kernel takes a compile-time BATCH flag that adds a grid dimension (blockIdx.y = cloud for the
+// layout and count, = (cloud, crop) pair for the gather, = crop for the edge filter, = crop run for the uncrop).  The
+// single-cloud entry points instantiate BATCH = false, whose code is the code from before the flag.
 #include <math.h>
 #include "psam_common.cuh"
 #include "../../include/psam_b200.h"
@@ -62,9 +66,20 @@ __device__ __forceinline__ bool in_box(float x, float y, float z, const float* b
     return b[0] <= x && x <= b[3] && b[1] <= y && y <= b[4] && b[2] <= z && z <= b[5];
 }
 
+// BATCH: cloud blockIdx.y of B clouds [B, N, 3] (N = N_max), its first clamp(lengths[b], 0, N) points when lengths is given;
+// boxes [B, T, 6], counts [B, T].  !BATCH is psam_crop_layout_f32's single cloud (lengths unused).
+template <bool BATCH>
 __global__ void __launch_bounds__(kLayoutThreads) crop_layout_kernel(const float* __restrict__ xyz, int N, int layers, float r,
-                                                                     float* __restrict__ boxes, int* __restrict__ counts) {
+                                                                     float* __restrict__ boxes, int* __restrict__ counts,
+                                                                     const int* __restrict__ lengths) {
     psam::pdl_prologue();
+    if constexpr (BATCH) {
+        const int b = blockIdx.y, T = crop_total(layers);
+        xyz += (size_t)b * N * 3;
+        boxes += (size_t)b * T * 6;
+        counts += (size_t)b * T;
+        if (lengths) N = min(max(lengths[b], 0), N);
+    }
     extern __shared__ float sbox[];  // [T, 6]
     __shared__ float red[6][kLayoutThreads / 32];
     __shared__ float bb[6];
@@ -119,9 +134,18 @@ __global__ void __launch_bounds__(kLayoutThreads) crop_layout_kernel(const float
     }
 }
 
+template <bool BATCH>
 __global__ void __launch_bounds__(kCountThreads) crop_count_kernel(const float* __restrict__ xyz, int N, int T,
-                                                                   const float* __restrict__ boxes, int* __restrict__ counts) {
+                                                                   const float* __restrict__ boxes, int* __restrict__ counts,
+                                                                   const int* __restrict__ lengths) {
     psam::pdl_prologue();
+    if constexpr (BATCH) {  // cloud blockIdx.y, as crop_layout_kernel<true>: padded rows are never read
+        const int b = blockIdx.y;
+        xyz += (size_t)b * N * 3;
+        boxes += (size_t)b * T * 6;
+        counts += (size_t)b * T;
+        if (lengths) N = min(max(lengths[b], 0), N);
+    }
     extern __shared__ float cbox[];  // [T, 6] boxes, then T counters (-1: duplicate crop, not counted)
     int* scnt = reinterpret_cast<int*>(cbox + 6 * T);
     for (int e = threadIdx.x; e < 6 * T; e += blockDim.x) cbox[e] = boxes[e];
@@ -150,10 +174,52 @@ __device__ __forceinline__ void crop_centre(const float* box, float (&c)[3]) {
     for (int a = 0; a < 3; ++a) c[a] = __fmul_rn(__fadd_rn(box[a], box[3 + a]), 0.5f);
 }
 
+// Pair blockIdx.y of the batched gather: pairs [3, P] holds the clouds, crops and counts.  Returns its cloud, crop and count,
+// and turns N (N_max on entry) into the number of the cloud's points to scan; a pair outside its ranges scans none and has
+// count 0 (its rows stay zero).
+__device__ __forceinline__ void gather_pair(const int* __restrict__ pairs, int P, int B, int n_crops, int n_max,
+                                            const int* __restrict__ lengths, int& N, int& crop, int& count, int& cloud) {
+    const int p = blockIdx.y;
+    cloud = pairs[p];
+    crop = pairs[P + p];
+    count = pairs[2 * P + p];
+    if (cloud < 0 || cloud >= B || crop < 0 || crop >= n_crops || count < 0 || count > n_max) {
+        cloud = crop = count = N = 0;
+        return;
+    }
+    if (lengths) N = min(max(lengths[cloud], 0), N);
+}
+
+// BATCH: pair blockIdx.y of the batched gather (gather_pair); `box` is then the boxes [B, n_crops, 6] of every cloud, and the
+// pair's rows [count, n_max) of idx_out / xyz_out / rgb_out [P, n_max(, 3)] are zeroed here (the write kernel fills the
+// others).  !BATCH is psam_crop_gather_f32's single crop (the batch arguments unused).
+template <bool BATCH>
 __global__ void __launch_bounds__(kChunk) crop_gather_count_kernel(const float* __restrict__ xyz, int N, const float* __restrict__ box,
                                                                    int* __restrict__ chunk_cnt, uint32_t* __restrict__ chunk_max,
-                                                                   uint32_t* __restrict__ edge, int We) {
+                                                                   uint32_t* __restrict__ edge, int We, const int* __restrict__ pairs,
+                                                                   int P, int B, int n_crops, int n_max, const int* __restrict__ lengths,
+                                                                   int* __restrict__ idx_out, float* __restrict__ xyz_out,
+                                                                   float* __restrict__ rgb_out) {
     psam::pdl_prologue();
+    if constexpr (BATCH) {
+        int crop, count, cloud;
+        const int N_max = N;
+        gather_pair(pairs, P, B, n_crops, n_max, lengths, N, crop, count, cloud);
+        xyz += (size_t)cloud * N_max * 3;
+        box += ((size_t)cloud * n_crops + crop) * 6;
+        const size_t p = blockIdx.y;
+        chunk_cnt += p * gridDim.x;
+        chunk_max += p * gridDim.x;
+        edge += p * We;
+        for (int q = count + blockIdx.x * kChunk + threadIdx.x; q < n_max; q += gridDim.x * kChunk) {
+            idx_out[p * n_max + q] = 0;
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                xyz_out[(p * n_max + q) * 3 + a] = 0.f;
+                rgb_out[(p * n_max + q) * 3 + a] = 0.f;
+            }
+        }
+    }
     __shared__ int wc[kChunk / 32];
     __shared__ float wm[kChunk / 32];
     const int i = blockIdx.x * kChunk + threadIdx.x;
@@ -190,13 +256,34 @@ __global__ void __launch_bounds__(kChunk) crop_gather_count_kernel(const float* 
     for (int w = blockIdx.x * kChunk + threadIdx.x; w < We; w += gridDim.x * kChunk) edge[w] = 0u;
 }
 
+// BATCH: pair blockIdx.y (gather_pair); `bbox` is then the boxes [B, n_crops, 6] of every cloud, and the outputs are the
+// pair's rows of idx_out / xyz_out / rgb_out [P, n_max(, 3)] and edge [P, We].
+template <bool BATCH>
 __global__ void __launch_bounds__(kChunk) crop_gather_write_kernel(const float* __restrict__ xyz, const float* __restrict__ rgb, int N,
                                                                    const float* __restrict__ bbox, const float* __restrict__ box,
                                                                    float margin, int n_out, const int* __restrict__ chunk_cnt,
                                                                    const uint32_t* __restrict__ chunk_max, int nchunks,
                                                                    int* __restrict__ idx_out, float* __restrict__ xyz_out,
-                                                                   float* __restrict__ rgb_out, uint32_t* __restrict__ edge) {
+                                                                   float* __restrict__ rgb_out, uint32_t* __restrict__ edge,
+                                                                   const int* __restrict__ pairs, int P, int B, int n_crops,
+                                                                   int n_max, const int* __restrict__ lengths, int We) {
     psam::pdl_prologue();
+    if constexpr (BATCH) {
+        int crop, cloud;
+        const int N_max = N;
+        gather_pair(pairs, P, B, n_crops, n_max, lengths, N, crop, n_out, cloud);
+        xyz += (size_t)cloud * N_max * 3;
+        rgb += (size_t)cloud * N_max * 3;
+        bbox += (size_t)cloud * n_crops * 6;
+        box = bbox + (size_t)crop * 6;
+        const size_t p = blockIdx.y;
+        chunk_cnt += p * nchunks;
+        chunk_max += p * nchunks;
+        idx_out += p * n_max;
+        xyz_out += p * n_max * 3;
+        rgb_out += p * n_max * 3;
+        edge += p * We;
+    }
     __shared__ int wpre[kChunk / 32 + 1];
     __shared__ int red_s[kChunk / 32];
     __shared__ float red_m[kChunk / 32];
@@ -258,9 +345,17 @@ __global__ void __launch_bounds__(kChunk) crop_gather_write_kernel(const float* 
     if (near) atomicOr(edge + (pos >> 5), 1u << (pos & 31));
 }
 
+// BATCH: crop blockIdx.y of bits [T, K, W], edge [T, W] and score [T, K].
+template <bool BATCH>
 __global__ void __launch_bounds__(kFilterWarps * 32) crop_edge_filter_kernel(const uint32_t* __restrict__ bits, int K, int W,
                                                                              const uint32_t* __restrict__ edge, float* __restrict__ score) {
     psam::pdl_prologue();
+    if constexpr (BATCH) {
+        const size_t t = blockIdx.y;
+        bits += t * K * W;
+        edge += t * W;
+        score += t * K;
+    }
     const int lane = threadIdx.x & 31;
     for (int k = blockIdx.x * kFilterWarps + (threadIdx.x >> 5); k < K; k += gridDim.x * kFilterWarps) {
         uint32_t hit = 0;
@@ -269,18 +364,65 @@ __global__ void __launch_bounds__(kFilterWarps * 32) crop_edge_filter_kernel(con
     }
 }
 
+// BATCH: run blockIdx.y of runs[] supplies the crop's arguments, and the outputs are its cloud's rows of [B, cloud_rows(, Wg)];
+// the offset is the exclusive prefix of the keep counts of the cloud's earlier runs (runs[first .. blockIdx.y)), and only the
+// cloud's last run writes its lifted count and overflow flag.  !BATCH is psam_crop_uncrop (runs / cloud_rows / lifted unused).
+template <bool BATCH>
 __global__ void __launch_bounds__(kUncropThreads) crop_uncrop_kernel(
     const uint32_t* __restrict__ bits, const int* __restrict__ area, const float* __restrict__ score,
     const float* __restrict__ stability, int W, const int* __restrict__ keep, const int* __restrict__ keep_count,
     const int* __restrict__ idx, int n, const long long* __restrict__ prompt_index, int slots, int crop, float layer_score,
     int Wg, int capacity, const int* __restrict__ offset_in, int* __restrict__ offset_out, uint32_t* __restrict__ gbits,
     int* __restrict__ garea, float* __restrict__ giou, float* __restrict__ gstab, long long* __restrict__ gprompt,
-    int* __restrict__ gslot, int* __restrict__ gcrop, float* __restrict__ gscore, int* __restrict__ overflow) {
+    int* __restrict__ gslot, int* __restrict__ gcrop, float* __restrict__ gscore, int* __restrict__ overflow,
+    const psam_crop_run* __restrict__ runs, int cloud_rows, int* __restrict__ lifted) {
     psam::pdl_prologue();
-    const int count = *keep_count, base = *offset_in;
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        *offset_out = base + count;
-        if (base + count > capacity) *overflow = 1;
+    int count, base;
+    if constexpr (BATCH) {
+        __shared__ int red[kUncropThreads / 32];
+        const psam_crop_run& r = runs[blockIdx.y];
+        bits = r.bits;
+        area = r.area;
+        score = r.score;
+        stability = r.stability;
+        W = r.W;
+        keep = r.keep;
+        idx = r.idx;
+        n = r.n;
+        prompt_index = r.prompt_index;
+        slots = r.slots;
+        crop = r.crop;
+        layer_score = r.layer_score;
+        capacity = min(r.capacity, cloud_rows);
+        const size_t c = r.cloud, rows = (size_t)c * cloud_rows;
+        gbits += rows * Wg;
+        garea += rows;
+        giou += rows;
+        gstab += rows;
+        gprompt += rows;
+        gslot += rows;
+        gcrop += rows;
+        gscore += rows;
+        int pre = 0;
+        for (int u = r.first + threadIdx.x; u < (int)blockIdx.y; u += blockDim.x) pre += *runs[u].keep_count;
+        pre = __reduce_add_sync(0xffffffffu, pre);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = pre;
+        __syncthreads();
+        base = 0;
+#pragma unroll
+        for (int w = 0; w < kUncropThreads / 32; ++w) base += red[w];
+        count = *r.keep_count;
+        if (blockIdx.x == 0 && threadIdx.x == 0 && r.last) {
+            lifted[c] = base + count;
+            overflow[c] = base + count > capacity ? 1 : 0;
+        }
+    } else {
+        count = *keep_count;
+        base = *offset_in;
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            *offset_out = base + count;
+            if (base + count > capacity) *overflow = 1;
+        }
     }
     for (int p = blockIdx.x; p < count; p += gridDim.x) {
         const int dst = base + p;
@@ -322,12 +464,12 @@ extern "C" int psam_crop_layout_f32(const float* xyz, int N, int n_layers, float
     if (!xyz || !boxes || !counts || N <= 0 || n_layers < 0 || n_layers > kCropMaxLayers) return PSAM_ERR_ARG;
     if (!(overlap_ratio >= 0.f && overlap_ratio < 1.f)) return PSAM_ERR_ARG;
     const int T = crop_total(n_layers);
-    PSAM_CUDA_TRY(psam::launch(crop_layout_kernel, dim3(1), dim3(kLayoutThreads), (size_t)T * 6 * sizeof(float), stream, xyz, N,
-                               n_layers, overlap_ratio, boxes, counts));
+    PSAM_CUDA_TRY(psam::launch(crop_layout_kernel<false>, dim3(1), dim3(kLayoutThreads), (size_t)T * 6 * sizeof(float), stream, xyz,
+                               N, n_layers, overlap_ratio, boxes, counts, (const int*)nullptr));
     PSAM_LAUNCH_CHECK();
     const int grid = min(psam::ceil_div(N, kCountThreads), kCountMaxBlocks);
-    PSAM_CUDA_TRY(psam::launch(crop_count_kernel, dim3(grid), dim3(kCountThreads), (size_t)T * 7 * sizeof(float), stream, xyz, N, T,
-                               (const float*)boxes, counts));
+    PSAM_CUDA_TRY(psam::launch(crop_count_kernel<false>, dim3(grid), dim3(kCountThreads), (size_t)T * 7 * sizeof(float), stream, xyz, N,
+                               T, (const float*)boxes, counts, (const int*)nullptr));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }
@@ -347,12 +489,13 @@ extern "C" int psam_crop_gather_f32(const float* xyz, const float* rgb, int N, c
     int* chunk_cnt = static_cast<int*>(workspace);
     uint32_t* chunk_max = reinterpret_cast<uint32_t*>(static_cast<char*>(workspace) + (size_t)psam::ceil_div(nchunks, 4) * 16);
     const float* box = boxes + (size_t)crop * 6;
-    PSAM_CUDA_TRY(psam::launch(crop_gather_count_kernel, dim3(nchunks), dim3(kChunk), (size_t)0, stream, xyz, N, box, chunk_cnt,
-                               chunk_max, edge, psam::ceil_div(n_out, 32)));
+    PSAM_CUDA_TRY(psam::launch(crop_gather_count_kernel<false>, dim3(nchunks), dim3(kChunk), (size_t)0, stream, xyz, N, box,
+                               chunk_cnt, chunk_max, edge, psam::ceil_div(n_out, 32), (const int*)nullptr, 0, 0, 0, 0,
+                               (const int*)nullptr, (int*)nullptr, (float*)nullptr, (float*)nullptr));
     PSAM_LAUNCH_CHECK();
-    PSAM_CUDA_TRY(psam::launch(crop_gather_write_kernel, dim3(nchunks), dim3(kChunk), (size_t)0, stream, xyz, rgb, N, boxes, box,
-                               edge_margin, n_out, (const int*)chunk_cnt, (const uint32_t*)chunk_max, nchunks, idx_out, xyz_out,
-                               rgb_out, edge));
+    PSAM_CUDA_TRY(psam::launch(crop_gather_write_kernel<false>, dim3(nchunks), dim3(kChunk), (size_t)0, stream, xyz, rgb, N, boxes,
+                               box, edge_margin, n_out, (const int*)chunk_cnt, (const uint32_t*)chunk_max, nchunks, idx_out,
+                               xyz_out, rgb_out, edge, (const int*)nullptr, 0, 0, 0, 0, (const int*)nullptr, 0));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }
@@ -361,7 +504,8 @@ extern "C" int psam_crop_edge_filter(const uint32_t* bits, int K, int W, const u
     if (K < 0 || (K > 0 && (!bits || !edge || !score || W <= 0))) return PSAM_ERR_ARG;
     if (K == 0) return PSAM_OK;
     const int grid = min(psam::ceil_div(K, kFilterWarps), 1024);
-    PSAM_CUDA_TRY(psam::launch(crop_edge_filter_kernel, dim3(grid), dim3(kFilterWarps * 32), (size_t)0, stream, bits, K, W, edge, score));
+    PSAM_CUDA_TRY(psam::launch(crop_edge_filter_kernel<false>, dim3(grid), dim3(kFilterWarps * 32), (size_t)0, stream, bits, K, W, edge,
+                               score));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }
@@ -378,9 +522,81 @@ extern "C" int psam_crop_uncrop(const uint32_t* bits, const int* area, const flo
         capacity < 1 || capacity > 16384)
         return PSAM_ERR_ARG;
     const int grid = min(K, kUncropMaxBlocks);
-    PSAM_CUDA_TRY(psam::launch(crop_uncrop_kernel, dim3(grid), dim3(kUncropThreads), (size_t)0, stream, bits, area, score, stability,
-                               W, keep, keep_count, idx, n, prompt_index, slots, crop, layer_score, Wg, capacity, offset_in,
-                               offset_out, gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore, overflow));
+    PSAM_CUDA_TRY(psam::launch(crop_uncrop_kernel<false>, dim3(grid), dim3(kUncropThreads), (size_t)0, stream, bits, area, score,
+                               stability, W, keep, keep_count, idx, n, prompt_index, slots, crop, layer_score, Wg, capacity,
+                               offset_in, offset_out, gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore, overflow,
+                               (const psam_crop_run*)nullptr, 0, (int*)nullptr));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" size_t psam_crop_run_bytes(void) { return sizeof(psam_crop_run); }
+
+extern "C" int psam_crop_layout_batched_f32(const float* xyz, const int* lengths, int B, int N_max, int n_layers, float overlap_ratio,
+                                            float* boxes, int* counts, cudaStream_t stream) {
+    if (!xyz || !boxes || !counts || B < 1 || B > 65535 || N_max <= 0 || n_layers < 0 || n_layers > kCropMaxLayers) return PSAM_ERR_ARG;
+    if (!(overlap_ratio >= 0.f && overlap_ratio < 1.f)) return PSAM_ERR_ARG;
+    const int T = crop_total(n_layers);
+    PSAM_CUDA_TRY(psam::launch(crop_layout_kernel<true>, dim3(1, B), dim3(kLayoutThreads), (size_t)T * 6 * sizeof(float), stream,
+                               xyz, N_max, n_layers, overlap_ratio, boxes, counts, lengths));
+    PSAM_LAUNCH_CHECK();
+    const int grid = min(psam::ceil_div(N_max, kCountThreads), kCountMaxBlocks);
+    PSAM_CUDA_TRY(psam::launch(crop_count_kernel<true>, dim3(grid, B), dim3(kCountThreads), (size_t)T * 7 * sizeof(float), stream,
+                               xyz, N_max, T, (const float*)boxes, counts, lengths));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" size_t psam_crop_gather_batched_workspace_bytes(int P, int N_max) {
+    if (P < 1 || P > 65535 || N_max <= 0) return 0;
+    return (size_t)P * psam::ceil_div(psam::ceil_div(N_max, kChunk), 4) * 32;
+}
+
+extern "C" int psam_crop_gather_batched_f32(const float* xyz, const float* rgb, const int* lengths, int B, int N_max, const float* boxes,
+                                            int n_crops, const int* pairs, int P, int n_max, float edge_margin, int* idx_out,
+                                            float* xyz_out, float* rgb_out, uint32_t* edge, void* workspace, cudaStream_t stream) {
+    if (!xyz || !rgb || !boxes || !pairs || !idx_out || !xyz_out || !rgb_out || !edge || !workspace) return PSAM_ERR_ARG;
+    if (B < 1 || N_max <= 0 || n_crops < 1 || P < 1 || P > 65535 || n_max < 1 || n_max > N_max || !(edge_margin >= 0.f))
+        return PSAM_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(workspace) & 15) return PSAM_ERR_ARG;
+    const int nchunks = psam::ceil_div(N_max, kChunk), We = psam::ceil_div(n_max, 32);
+    int* chunk_cnt = static_cast<int*>(workspace);
+    uint32_t* chunk_max = reinterpret_cast<uint32_t*>(static_cast<char*>(workspace) + (size_t)P * psam::ceil_div(nchunks, 4) * 16);
+    PSAM_CUDA_TRY(psam::launch(crop_gather_count_kernel<true>, dim3(nchunks, P), dim3(kChunk), (size_t)0, stream, xyz, N_max, boxes,
+                               chunk_cnt, chunk_max, edge, We, pairs, P, B, n_crops, n_max, lengths, idx_out, xyz_out, rgb_out));
+    PSAM_LAUNCH_CHECK();
+    PSAM_CUDA_TRY(psam::launch(crop_gather_write_kernel<true>, dim3(nchunks, P), dim3(kChunk), (size_t)0, stream, xyz, rgb, N_max,
+                               boxes, boxes, edge_margin, 0, (const int*)chunk_cnt, (const uint32_t*)chunk_max, nchunks, idx_out,
+                               xyz_out, rgb_out, edge, pairs, P, B, n_crops, n_max, lengths, We));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" int psam_crop_edge_filter_batched(const uint32_t* bits, int T, int K, int W, const uint32_t* edge, float* score,
+                                             cudaStream_t stream) {
+    if (T < 1 || T > 65535 || K < 0 || (K > 0 && (!bits || !edge || !score || W <= 0))) return PSAM_ERR_ARG;
+    if (K == 0) return PSAM_OK;
+    const int grid = min(psam::ceil_div(K, kFilterWarps), 1024);
+    PSAM_CUDA_TRY(psam::launch(crop_edge_filter_kernel<true>, dim3(grid, T), dim3(kFilterWarps * 32), (size_t)0, stream, bits, K, W,
+                               edge, score));
+    PSAM_LAUNCH_CHECK();
+    return PSAM_OK;
+}
+
+extern "C" int psam_crop_uncrop_batched(const psam_crop_run* runs, int R, int K_max, int B, int N_max, int Wg, int cloud_rows,
+                                        uint32_t* gbits, int* garea, float* giou, float* gstab, long long* gprompt, int* gslot,
+                                        int* gcrop, float* gscore, int* lifted, int* overflow, cudaStream_t stream) {
+    if (!runs || !gbits || !garea || !giou || !gstab || !gprompt || !gslot || !gcrop || !gscore || !lifted || !overflow)
+        return PSAM_ERR_ARG;
+    if (R < 1 || R > 65535 || K_max < 1 || B < 1 || N_max < 1 || Wg < psam::ceil_div(N_max, 32) || cloud_rows < 1 ||
+        cloud_rows > 16384)
+        return PSAM_ERR_ARG;
+    const int grid = min(K_max, max(16, 2 * kUncropMaxBlocks / R));
+    PSAM_CUDA_TRY(psam::launch(crop_uncrop_kernel<true>, dim3(grid, R), dim3(kUncropThreads), (size_t)0, stream, (const uint32_t*)nullptr,
+                               (const int*)nullptr, (const float*)nullptr, (const float*)nullptr, 0, (const int*)nullptr,
+                               (const int*)nullptr, (const int*)nullptr, 0, (const long long*)nullptr, 0, 0, 0.f, Wg, 0,
+                               (const int*)nullptr, (int*)nullptr, gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore, overflow,
+                               runs, cloud_rows, lifted));
     PSAM_LAUNCH_CHECK();
     return PSAM_OK;
 }

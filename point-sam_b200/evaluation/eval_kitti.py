@@ -18,6 +18,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from pc_sam.model.loss import compute_iou  # noqa: E402
 from pc_sam.utils.ply import normalize_colors, normalize_points, read_ply, vertex_count  # noqa: E402
+from psam_b200.parallel import plan_eval_batches  # noqa: E402,F401  (the batch plan, shared with the mask generator)
 
 
 def transform_fn(x: Dict[str, np.ndarray], device="cuda") -> Dict[str, torch.Tensor]:
@@ -80,32 +81,6 @@ def set_group_shape(model, num_points: int):
     if g is None:
         return
     g.num_groups, g.group_size = group_shape_for(num_points)
-
-
-def plan_eval_batches(sizes: Sequence[int], keys: Sequence[Hashable], batch_size: int,
-                      max_batch_points: int) -> List[List[int]]:
-    """Batches of crop indices for forward_varlen.  Crops are grouped by key (their group shape: crops of different
-    shapes need different G / K and never share a batch), each group is sorted by size so that the padding stays small,
-    and runs of at most batch_size crops with len(batch) * N_max <= max_batch_points are cut from it (a crop larger than
-    the cap runs alone).  The cap bounds the decoder's upscaling input, B * M * N_max * Du * 4 bytes.  Groups come in
-    order of first appearance; every crop appears exactly once."""
-    if batch_size < 1 or max_batch_points < 1:
-        raise ValueError(f"batch_size ({batch_size}) and max_batch_points ({max_batch_points}) must be >= 1")
-    if len(sizes) != len(keys):
-        raise ValueError(f"{len(sizes)} sizes and {len(keys)} keys")
-    groups: Dict[Hashable, List[int]] = {}
-    for i, k in enumerate(keys):
-        groups.setdefault(k, []).append(i)
-    batches: List[List[int]] = []
-    for idx in groups.values():
-        cur: List[int] = []
-        for i in sorted(idx, key=lambda j: (sizes[j], j)):
-            if cur and (len(cur) + 1 > batch_size or (len(cur) + 1) * sizes[i] > max_batch_points):
-                batches.append(cur)
-                cur = []
-            cur.append(i)
-        batches.append(cur)
-    return batches
 
 
 def _run_batch(model, data: List[Dict[str, torch.Tensor]]):

@@ -68,7 +68,8 @@ EXPORTS = [
     "psam_mask_regions_batched_workspace_bytes", "psam_mask_regions_batched",
     "psam_fps_varlen_f32", "psam_knn_varlen_f32", "psam_mask_candidates_varlen_f32", "psam_mask_regions_varlen",
     "psam_crop_total", "psam_crop_layout_f32", "psam_crop_gather_workspace_bytes", "psam_crop_gather_f32", "psam_crop_edge_filter",
-    "psam_crop_uncrop",
+    "psam_crop_uncrop", "psam_crop_layout_batched_f32", "psam_crop_gather_batched_workspace_bytes", "psam_crop_gather_batched_f32",
+    "psam_crop_edge_filter_batched", "psam_crop_run_bytes", "psam_crop_uncrop_batched",
     "psam_mesh_sample_workspace_bytes", "psam_mesh_sample_f32", "psam_mesh_face_centers_f32", "psam_mask_lift", "psam_mask_label_map",
     "psam_nn_grid_workspace_bytes", "psam_nn_grid_f32", "psam_voxel_subsample_workspace_bytes", "psam_voxel_subsample_f32",
     "psam_version",
@@ -99,6 +100,10 @@ def lib():
         L.psam_mask_regions_batched_workspace_bytes.argtypes = [i, i, i]
         L.psam_crop_gather_workspace_bytes.restype = c_size_t
         L.psam_crop_gather_workspace_bytes.argtypes = [i]
+        L.psam_crop_gather_batched_workspace_bytes.restype = c_size_t
+        L.psam_crop_gather_batched_workspace_bytes.argtypes = [i, i]
+        L.psam_crop_run_bytes.restype = c_size_t
+        L.psam_crop_run_bytes.argtypes = []
         L.psam_mesh_sample_workspace_bytes.restype = c_size_t
         L.psam_mesh_sample_workspace_bytes.argtypes = [i]
         L.psam_nn_grid_workspace_bytes.restype = c_size_t
@@ -150,6 +155,10 @@ def lib():
             "psam_crop_gather_f32": [p, p, i, p, i, i, f, i, p, p, p, p, p, p],
             "psam_crop_edge_filter": [p, i, i, p, p, p],
             "psam_crop_uncrop": [p, p, p, p, i, i, p, p, p, i, p, i, i, f, i, i, i, p, p, p, p, p, p, p, p, p, p, p, p],
+            "psam_crop_layout_batched_f32": [p, p, i, i, i, f, p, p, p],
+            "psam_crop_gather_batched_f32": [p, p, p, i, i, p, i, p, i, i, f, p, p, p, p, p, p],
+            "psam_crop_edge_filter_batched": [p, i, i, i, p, p, p],
+            "psam_crop_uncrop_batched": [p, i, i, i, i, i, i, p, p, p, p, p, p, p, p, p, p, p],
             "psam_mesh_sample_f32": [p, i, p, i, i, ctypes.c_uint64, p, p, p, i, i, i, p, p, p, p, p, p],
             "psam_mesh_face_centers_f32": [p, i, p, i, p, p],
             "psam_mask_lift": [p, i, i, i, p, i, i, p, p, p],

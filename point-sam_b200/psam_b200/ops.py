@@ -8,6 +8,7 @@ from __future__ import annotations
 from ctypes import byref
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import native as nv
@@ -598,6 +599,120 @@ def crop_uncrop(cand, keep: torch.Tensor, keep_count: torch.Tensor, idx: torch.T
                                        float(layer_score), int(N), Wg, cap, nv.ptr(offsets[k:]), nv.ptr(offsets[k + 1:]), nv.ptr(gbits),
                                        nv.ptr(garea), nv.ptr(giou), nv.ptr(gstab), nv.ptr(gprompt), nv.ptr(gslot), nv.ptr(gcrop),
                                        nv.ptr(gscore), nv.ptr(overflow), nv.stream()), "crop_uncrop")
+
+
+def _host_to_device(a: np.ndarray, dev) -> torch.Tensor:
+    """A small host table on the device without a host synchronisation (pinned memory, asynchronous copy)."""
+    host = torch.from_numpy(np.ascontiguousarray(a))
+    return (host.pin_memory() if dev.type == "cuda" else host).to(dev, non_blocking=True)
+
+
+def crop_layout_batched(xyz: torch.Tensor, n_layers: int, overlap_ratio: float, lengths: Optional[torch.Tensor] = None):
+    """crop_layout on each cloud of xyz [B, N_max, 3] in one pair of launches (psam_crop_layout_batched_f32).  lengths [B]
+    int32 (device): cloud b is its first lengths[b] rows.  Returns (boxes [B, T, 6], counts [B, T]) on the device."""
+    if xyz.dim() != 3 or xyz.shape[2] != 3:
+        raise ValueError(f"crop_layout_batched: xyz must be [B, N, 3], got {tuple(xyz.shape)}")
+    x = xyz.float().contiguous()
+    B, N, dev = x.shape[0], x.shape[1], x.device
+    T = crop_total(n_layers)
+    if lengths is not None:
+        lengths = _lengths(lengths, B, "crop_layout_batched")
+    boxes = torch.empty((B, T, 6), dtype=torch.float32, device=dev)
+    counts = torch.empty((B, T), dtype=torch.int32, device=dev)
+    nv.check(nv.lib().psam_crop_layout_batched_f32(nv.ptr(x), nv.ptr(lengths), B, N, int(n_layers), float(overlap_ratio), nv.ptr(boxes),
+                                                   nv.ptr(counts), nv.stream()), "crop_layout_batched")
+    return boxes, counts
+
+
+def crop_gather_batched(xyz: torch.Tensor, rgb: torch.Tensor, boxes: torch.Tensor, pairs, edge_margin: float,
+                        lengths: Optional[torch.Tensor] = None):
+    """The crop clouds of P (cloud, crop, count) pairs (host ints; count = the crop's entry of crop_layout_batched's counts)
+    as one padded batch (psam_crop_gather_batched_f32): xyz / rgb [B, N_max, 3] with lengths [B] as for the layout, boxes
+    [B, T, 6].  Returns (idx [P, n_max] int32, xyz [P, n_max, 3] renormalised, rgb [P, n_max, 3], edge [P, mask_words(n_max)]
+    int32, counts [P] int32 on the device: the `lengths` of the padded batch), n_max = the largest count; row p equals
+    crop_gather of its pair, and its rows past the count are 0.  Nothing waits for the device."""
+    x, c = xyz.float().contiguous(), rgb.float().contiguous()
+    if x.dim() != 3 or x.shape[2] != 3 or c.shape != x.shape:
+        raise ValueError(f"crop_gather_batched: xyz {tuple(x.shape)} and rgb {tuple(c.shape)} must both be [B, N, 3]")
+    B, N, dev = x.shape[0], x.shape[1], x.device
+    if boxes.dim() != 3 or boxes.shape[0] != B or boxes.shape[2] != 6:
+        raise ValueError(f"crop_gather_batched: boxes must be [{B}, T, 6], got {tuple(boxes.shape)}")
+    table = np.asarray(pairs, dtype=np.int32).reshape(-1, 3)
+    P = table.shape[0]
+    if P < 1 or table[:, 2].min() < 1:
+        raise ValueError("crop_gather_batched: need at least one pair, each with a count >= 1")
+    n_max = int(table[:, 2].max())
+    if lengths is not None:
+        lengths = _lengths(lengths, B, "crop_gather_batched")
+    table = _host_to_device(table.T, dev)
+    idx = torch.empty((P, n_max), dtype=torch.int32, device=dev)
+    xo = torch.empty((P, n_max, 3), dtype=torch.float32, device=dev)
+    co = torch.empty((P, n_max, 3), dtype=torch.float32, device=dev)
+    edge = torch.empty((P, mask_words(n_max)), dtype=torch.int32, device=dev)
+    ws = torch.empty(max(1, nv.lib().psam_crop_gather_batched_workspace_bytes(P, N)), dtype=torch.uint8, device=dev)
+    nv.check(nv.lib().psam_crop_gather_batched_f32(nv.ptr(x), nv.ptr(c), nv.ptr(lengths), B, N, nv.ptr(boxes.contiguous()), boxes.shape[1],
+                                                   nv.ptr(table), P, n_max, float(edge_margin), nv.ptr(idx), nv.ptr(xo), nv.ptr(co),
+                                                   nv.ptr(edge), nv.ptr(ws), nv.stream()), "crop_gather_batched")
+    return idx, xo, co, edge, table[2]
+
+
+def crop_edge_filter_batched(bits: torch.Tensor, score: torch.Tensor, edge: torch.Tensor):
+    """crop_edge_filter on each crop of bits [T, K, W], score [T, K] and edge [T, W] in one launch
+    (psam_crop_edge_filter_batched)."""
+    T, K, W = bits.shape
+    if tuple(edge.shape) != (T, W) or tuple(score.shape) != (T, K):
+        raise ValueError(f"crop_edge_filter_batched: edge {tuple(edge.shape)} and score {tuple(score.shape)} for bits {tuple(bits.shape)}")
+    nv.check(nv.lib().psam_crop_edge_filter_batched(nv.ptr(bits) if K else None, T, K, W, nv.ptr(edge) if K else None,
+                                                    nv.ptr(score) if K else None, nv.stream()), "crop_edge_filter_batched")
+
+
+# psam_crop_run of include/psam_b200.h
+CROP_RUN = np.dtype([("bits", "<u8"), ("area", "<u8"), ("score", "<u8"), ("stability", "<u8"), ("keep", "<u8"), ("keep_count", "<u8"),
+                     ("idx", "<u8"), ("prompt_index", "<u8"), ("K", "<i4"), ("W", "<i4"), ("n", "<i4"), ("slots", "<i4"), ("crop", "<i4"),
+                     ("cloud", "<i4"), ("first", "<i4"), ("last", "<i4"), ("layer_score", "<f4"), ("capacity", "<i4")])
+
+
+def crop_uncrop_batched(runs, out, N: int):
+    """The kept masks of every crop run of B clouds lifted to their clouds in one launch (psam_crop_uncrop_batched).
+    runs: per run a dict with cand = (bits [K', W], area, stability, score) of its candidates, keep [K] int32 and keep_count
+    [1] (its NMS), idx (int32, the crop's point indices in its cloud: n = idx.numel()), prompt_index (int64, crop-local), slots,
+    crop, layer, cloud and capacity (its cloud's); the runs of a cloud consecutive and in the cloud's crop order, every cloud
+    0 .. B-1 with at least one.  out = (gbits [B, cap, Wg] int32, area, iou, stability, prompt int64, slot, crop int32,
+    score fp32, each [B, cap]); N = the clouds' N_max.  Returns (lifted [B], overflow [B]) int32 on the device: each cloud's
+    kept count over all its runs and 1 where it exceeds the cloud's capacity.  The slices in `runs` must stay alive until the
+    launch has run (the caller holds them)."""
+    gbits, garea, giou, gstab, gprompt, gslot, gcrop, gscore = out
+    B, cap, Wg = gbits.shape
+    dev = gbits.device
+    if nv.lib().psam_crop_run_bytes() != CROP_RUN.itemsize:
+        raise RuntimeError(f"crop_uncrop_batched: psam_crop_run is {nv.lib().psam_crop_run_bytes()} bytes, the binding lays out "
+                           f"{CROP_RUN.itemsize}")
+    table = np.zeros(len(runs), dtype=CROP_RUN)
+    first, K_max = 0, 1
+    for r, run in enumerate(runs):
+        bits, area, stab, score = run["cand"]
+        if bits.dim() != 2 or not bits.is_contiguous() or run["idx"].dim() != 1:
+            raise ValueError("crop_uncrop_batched: each run's bits must be a contiguous [K, W] slice and its idx one row")
+        if r and runs[r - 1]["cloud"] != run["cloud"]:
+            first = r
+        last = r + 1 == len(runs) or runs[r + 1]["cloud"] != run["cloud"]
+        if not 0 <= run["cloud"] < B or not 1 <= run["capacity"] <= cap or (r and run["cloud"] < runs[r - 1]["cloud"]):
+            raise ValueError(f"crop_uncrop_batched: run {r} has cloud {run['cloud']} and capacity {run['capacity']} for {B} clouds of "
+                             f"{cap} rows (runs grouped by cloud in ascending order)")
+        keep = run["keep"]
+        K_max = max(K_max, keep.numel())
+        table[r] = (nv.ptr(bits), nv.ptr(area), nv.ptr(score), nv.ptr(stab), nv.ptr(keep), nv.ptr(run["keep_count"]), nv.ptr(run["idx"]),
+                    nv.ptr(run["prompt_index"]), keep.numel(), bits.shape[1], run["idx"].numel(), int(run["slots"]), int(run["crop"]),
+                    int(run["cloud"]), first, int(last), float(run["layer"]), int(run["capacity"]))
+    if sorted({int(r["cloud"]) for r in runs}) != list(range(B)):
+        raise ValueError(f"crop_uncrop_batched: every one of the {B} clouds needs at least one run")
+    dtable = _host_to_device(table.view(np.uint8), dev)
+    lifted = torch.empty(B, dtype=torch.int32, device=dev)
+    overflow = torch.empty(B, dtype=torch.int32, device=dev)
+    nv.check(nv.lib().psam_crop_uncrop_batched(nv.ptr(dtable), len(runs), K_max, B, int(N), Wg, cap, nv.ptr(gbits), nv.ptr(garea),
+                                               nv.ptr(giou), nv.ptr(gstab), nv.ptr(gprompt), nv.ptr(gslot), nv.ptr(gcrop), nv.ptr(gscore),
+                                               nv.ptr(lifted), nv.ptr(overflow), nv.stream()), "crop_uncrop_batched")
+    return lifted, overflow
 
 
 # ------------------------------------------------------------------------------------------------
