@@ -409,7 +409,8 @@ int psam_mask_candidates_varlen_f32(const float* logits, const float* iou_preds,
 /* Greedy mask-IoU non-maximum suppression over K <= 16384 candidate slots of W words each (the output of
  * psam_mask_candidates_f32).  Stands in for the duplicate-removal stage of SamAutomaticMaskGenerator._process_batch /
  * _process_crop (batched_nms on boxes), here on the masks themselves.
- * Candidates are ordered by (score descending, slot index ascending); -inf scores are dropped.  Walking that order, a
+ * Candidates are ordered by (score descending, slot index ascending); -inf scores are dropped.  NaN scores are dropped
+ * like -inf, and -0.0 ranks equal to +0.0 (the lower slot goes first).  Walking that order, a
  * candidate is kept unless an earlier kept one overlaps it with
  *   fp32(inter) / fp32(area_i + area_j - inter) > nms_thresh,   inter = popcount(bits_i & bits_j),
  * so the result is exact and bit-reproducible.  Three launches (order, pairwise suppression bits, greedy scan) and no

@@ -175,7 +175,8 @@ __global__ void __launch_bounds__(1024) nms_order_kernel(const float* __restrict
         if (i < K) {
             const float s = score[i];
             if (s > -INFINITY) {  // -inf (filtered) and NaN are dropped
-                uint32_t u = __float_as_uint(s);
+                // + 0: -0.0 becomes +0.0, so the two zeros share a key and the slot decides, as for any other tie
+                uint32_t u = __float_as_uint(__fadd_rn(s, 0.f));
                 u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);  // monotone in s
                 k = ((unsigned long long)(~u) << 32) | (uint32_t)i;  // ascending key = score descending, slot ascending
                 ++valid;
