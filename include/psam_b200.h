@@ -482,7 +482,10 @@ int psam_mask_regions_varlen(const uint32_t* bits, long long cloud_slots, const 
 /* Layout.  Layer 0 is the whole cloud.  Layer i >= 1 splits every axis a of the cloud's axis-aligned bounding box
  * [lo_a, hi_a] into n = 2^i crops.  Everything is fp32, every operation rounded on its own (no contraction), in this order:
  *   lo_a = min_n xyz[n, a], hi_a = max_n xyz[n, a]          (exact; NaN coordinates are ignored, and an axis with
- *                                                              nothing but NaN gives lo_a = +inf, hi_a = -inf)
+ *                                                              nothing but NaN gives lo_a = +inf, hi_a = -inf; -0.0
+ *                                                              orders below +0.0, so lo_a = -0.0 when the axis's smallest
+ *                                                              value is zero and one of its zeros is -0.0, and hi_a = +0.0
+ *                                                              when its largest is zero and one of its zeros is +0.0)
  *   L_a  = hi_a - lo_a
  *   o_a  = ((r * L_a) * 2) / n                                r = overlap_ratio
  *   s_a  = (L_a + o_a * (n - 1)) / n
@@ -609,7 +612,9 @@ int psam_crop_uncrop_batched(const psam_crop_run* runs, int R, int K_max, int B,
  *           a face is chosen with probability q_f / total and a weight-0 face never.
  *   point   r1 = (h_1 >> 40) * 2^-24, r2 = (h_2 >> 40) * 2^-24 (exact), v = sqrt(r1), w = (1 - v, v * (1 - r2), v * r2);
  *           p = (w0 * a + w1 * b) + w2 * c, then each axis clamped to [min, max] of the three vertices' coordinates (so the
- *           samples of a mesh inside [-1, 1] stay inside it).
+ *           samples of a mesh inside [-1, 1] stay inside it): min(max(p, min(min(a, b), c)), max(max(a, b), c)), where
+ *           min and max ignore a NaN operand and order -0.0 below +0.0 (so a p of either sign of zero inside the box is
+ *           kept as it is).
  *   colour  with texture [tex_h, tex_w, tex_c] uint8 (tex_c = 3 or 4) and uv [V, 2]: (tu, tv) = the uv interpolated like p
  *           (not clamped), texel x = floor(tu * tex_w + 0.5), y = floor((1 - tv) * tex_h + 0.5), each clamped into the image
  *           (a NaN gives 0); the colour is its first three channels / 255.  Otherwise with vertex_colors [V, 3]: interpolated

@@ -29,11 +29,15 @@ def crop_layers(n_layers: int):
 
 
 def bounding_box(xyz) -> np.ndarray:
-    """(lo, hi) per axis over the non-NaN coordinates; an all-NaN axis gives (+inf, -inf)."""
+    """(lo, hi) per axis over the non-NaN coordinates, -0.0 ordered below +0.0; an all-NaN axis gives (+inf, -inf)."""
     x = np.asarray(xyz, dtype=F).reshape(-1, 3)
     nan = np.isnan(x)
     lo = np.where(nan, F(np.inf), x).min(0, initial=F(np.inf))
     hi = np.where(nan, F(-np.inf), x).max(0, initial=F(-np.inf))
+    # ndarray.min / max return either zero when +0.0 and -0.0 meet, depending on the order of the elements
+    neg0, pos0 = ((x == 0) & np.signbit(x)).any(0), ((x == 0) & ~np.signbit(x)).any(0)
+    lo = np.where(lo == 0, np.where(neg0, F(-0.0), F(0.0)), lo)
+    hi = np.where(hi == 0, np.where(pos0, F(0.0), F(-0.0)), hi)
     return np.concatenate([lo, hi]).astype(F)
 
 

@@ -78,8 +78,20 @@ def _bary(w0, w1, w2, a, b, c):
     return (w0 * a + w1 * b) + w2 * c
 
 
+def _fmin(a, b):
+    """np.fmin with -0.0 ordered below +0.0 (np.fmin returns its second operand when the two compare equal)."""
+    zero = (a == 0) & (b == 0)
+    return np.where(zero, np.where(np.signbit(a) | np.signbit(b), F32(-0.0), F32(0.0)), np.fmin(a, b)).astype(F32)
+
+
+def _fmax(a, b):
+    """np.fmax with -0.0 ordered below +0.0."""
+    zero = (a == 0) & (b == 0)
+    return np.where(zero, np.where(np.signbit(a) & np.signbit(b), F32(-0.0), F32(0.0)), np.fmax(a, b)).astype(F32)
+
+
 def _clamp3(p, a, b, c):
-    return np.fmin(np.fmax(p, np.fmin(np.fmin(a, b), c)), np.fmax(np.fmax(a, b), c))
+    return _fmin(_fmax(p, _fmin(_fmin(a, b), c)), _fmax(_fmax(a, b), c))
 
 
 def texel(t: np.ndarray, n: int) -> np.ndarray:

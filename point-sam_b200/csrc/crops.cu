@@ -83,6 +83,7 @@ __global__ void __launch_bounds__(kLayoutThreads) crop_layout_kernel(const float
     extern __shared__ float sbox[];  // [T, 6]
     __shared__ float red[6][kLayoutThreads / 32];
     __shared__ float bb[6];
+    // fminf / fmaxf ignore NaN and order -0.0 below +0.0 (PTX min / max), so the box is the same in any reduction order
     float v[6] = {INFINITY, INFINITY, INFINITY, -INFINITY, -INFINITY, -INFINITY};
     for (int i = threadIdx.x; i < N; i += blockDim.x) {
 #pragma unroll

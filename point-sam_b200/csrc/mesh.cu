@@ -134,6 +134,7 @@ __device__ __forceinline__ float bary(float w0, float w1, float w2, float a, flo
     return __fadd_rn(__fadd_rn(__fmul_rn(w0, a), __fmul_rn(w1, b)), __fmul_rn(w2, c));
 }
 
+// fminf / fmaxf (PTX min / max) order -0.0 below +0.0, the header's rule: a zero p inside the box keeps its sign
 __device__ __forceinline__ float clamp3(float p, float a, float b, float c) {
     return fminf(fmaxf(p, fminf(fminf(a, b), c)), fmaxf(fmaxf(a, b), c));
 }
