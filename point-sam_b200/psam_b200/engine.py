@@ -3,7 +3,10 @@
 The modules in ``pc_sam.model`` only hold parameters (reference state-dict layout); their ``forward``
 methods call the ``run_*`` functions here.  Weights are re-packed (split-bf16, fused qkv, padded SwiGLU)
 lazily and cached per module; the cache is keyed on parameter storage/version so ``load_state_dict``,
-``safetensors.load_model`` and ``.cuda()`` are picked up automatically.
+``safetensors.load_model``, in-place updates of the parameters under ``torch.no_grad()`` and ``.cuda()`` are picked up
+automatically.  Two kinds of change are not: a write through ``p.data`` (``p.data.copy_(...)`` leaves ``p._version`` as it
+was), and assigning a LayerNorm's ``eps`` (an attribute, not a parameter).  Make either before the module's first call, or
+follow it with a real parameter update (``load_state_dict``).
 """
 from __future__ import annotations
 
