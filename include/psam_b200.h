@@ -715,6 +715,58 @@ size_t psam_voxel_subsample_workspace_bytes(int P);
 int psam_voxel_subsample_f32(const float* xyz, int P, int S, unsigned long long seed, long long* idx_out, long long* stats,
                              void* workspace, cudaStream_t stream);
 
+/* ---- decoder fine-tuning (csrc/train.cu) ------------------------------------------------------------------------------
+ * Training of mask_decoder on a frozen encoder: the reference's mask loss (pc_sam/model/loss.py:58-158) and the backward of
+ * the per-point mask head (mask_decoder.py:146-176).  No float atomics: every output is bitwise reproducible run to run. */
+
+/* Per (row z, mask c) statistics of compute_mask_loss over logits [Z,C,N] fp32 and gt [Z,N] (bytes, nonzero = inside):
+ * stats[z,c,:] = (sum_n focal, sum_n p t, sum_n p^2, sum_n t) with p = sigmoid(logit), focal = torchvision's
+ * sigmoid_focal_loss(alpha=-1, gamma=2) = BCE-with-logits * (1 - p_t)^2; counts[z,c,:] = (|pred & gt|, |pred | gt|) with
+ * pred = logit > 0 (compute_iou).  Every element and sum in fp64, stored as fp32 / int32.  One CTA per (z, c).
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_loss_stats(const float* logits, const unsigned char* gt, int Z, int C, int N, float* stats, int* counts,
+                         cudaStream_t stream);
+
+/* dlogits[z,c,n] = dloss[z,c] * d(focal_mean + 2 dice)[z,c] / dlogit[z,c,n], dice = 1 - (2 sum p t + 1e-3) / (sum p^2 + sum t
+ * + 1e-3), from psam_mask_loss_stats' stats.  A (z, c) with dloss == 0 (a mask the criterion did not select) is written as
+ * zeros without evaluating its terms.  Z * C <= 65535.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_mask_loss_grad(const float* logits, const unsigned char* gt, int Z, int C, int N, const float* stats, const float* dloss,
+                        float* dlogits, cudaStream_t stream);
+
+/* Inverse of the 3-NN interpolation index idx [B,N,3] (int64, values in [0, G); psam_knn3_interp_f32): per cloud b,
+ * offsets[b, g] .. offsets[b, g+1] (int32 [B, G+1]) delimit the entries e = n * 3 + k with idx[b,n,k] == g in entries
+ * (int32 [B, 3N]), in ascending e.  One CTA per cloud; a stable counting sort.  G <= 8192.  Bad arguments -> PSAM_ERR_ARG
+ * before any CUDA call. */
+int psam_interp_inverse(const long long* idx, int B, int N, int G, int* offsets, int* entries, cudaStream_t stream);
+
+/* Head backward, elementwise part.  p [Z*N, D] = output_upscaling[3] pre-activation (fp32), dm [Z,C,N] the gradient of the
+ * masks, hyper [Z,C,D]:  dp[z*N+n, d] = GELU'(p) * sum_c dm[z,c,n] hyper[z,c,d] as split-bf16 (row stride ldp_s, lo plane
+ * dp_plane elements after the hi plane), and partial sums over chunks of 128 points (K = psam_head_dp_chunks(N) chunks):
+ * part_hyper [Z, K, C, D] of dm * GELU(p) (-> dhyper) and part_b3 [Z, K, D] of dp (-> the bias gradient); psam_sum_partials
+ * finishes both.  C <= 8, D a multiple of 32 <= 1024, Z <= 65535.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_head_dp(const float* p, const float* dm, const float* hyper, int Z, int C, int N, int D, void* dp_hi, long long dp_plane,
+                 long long ldp_s, float* part_hyper, float* part_b3, cudaStream_t stream);
+int psam_head_dp_chunks(int N);
+
+/* Backward of psam_interp_ln_gelu: du [Z*N, D] holds dL/dy on entry and dL/dv on return (in place), v = the interpolated
+ * row before the LayerNorm; the interpolation and LayerNorm are recomputed with the forward's arithmetic.  part
+ * [ceil(Z*N / rows_per_block), 2, D] receives per-CTA partial sums of dgamma (row 0) and dbeta (row 1), each CTA covering
+ * rows_per_block consecutive rows; psam_sum_partials finishes them.  D in {128, 256, 512} (PSAM_ERR_UNSUPPORTED otherwise).
+ * Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_interp_ln_gelu_backward(const float* f, int Z, int rep, int G, int D, const long long* idx, const float* w, int N,
+                                 const float* gamma, const float* beta, float eps, float* du, float* part, int rows_per_block,
+                                 cudaStream_t stream);
+
+/* Backward of the 3-NN interpolation (interpolate_features, common.py:258-274) as a gather: df[z*G+g, :] = sum over the
+ * entries e of patch g of cloud b = z / rep (psam_interp_inverse, in its order) of w[b, e] * dv[z*N + e/3, :].  D a multiple of
+ * 128 <= 1024 (PSAM_ERR_UNSUPPORTED otherwise).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_interp_backward(const float* dv, int Z, int rep, int G, int D, const int* offsets, const int* entries, const float* w, int N,
+                         float* df, cudaStream_t stream);
+
+/* out[b*n + i] = sum_{s < S} part[(b*S + s)*n + i], in order s = 0, 1, ... with an fp64 accumulator: the fixed-order finish of
+ * every partial-sum buffer above (and of split-K GEMM partials).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+int psam_sum_partials(const float* part, int nb, int S, long long n, float* out, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

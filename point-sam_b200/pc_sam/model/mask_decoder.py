@@ -17,6 +17,7 @@ class AuxInputs:
     centers: torch.Tensor
     interp_index: torch.Tensor = None
     interp_weight: torch.Tensor = None
+    interp_inverse: tuple = None  # (interp_index, offsets, entries): its inverse for fine-tuning (psam_b200.train)
 
 
 class MLP(nn.Module):

@@ -1,7 +1,8 @@
 """PointCloudSAM with the reference API (/root/reference/pc_sam/model/pc_sam.py:20-196) plus the
 ``set_pointcloud`` / 4-argument ``predict_masks`` form that demo/app.py:198-205 calls.
 
-All computation runs in the sm_100a kernels behind ``psam_b200`` (no CPU / PyTorch fallback)."""
+All computation runs in the sm_90a kernels behind ``psam_b200`` (no CPU / PyTorch fallback).  Training mode fine-tunes
+mask_decoder on a frozen encoder (psam_b200.train); everything else is inference."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -272,18 +273,70 @@ class PointCloudSAM(nn.Module):
         evaluation/inference.py:67-68.  Prompts are sampled from the ground truth with the reference's
         sampler (pc_sam/model/common.py:287-474) restated in pc_sam.model.prompt_sampling."""
         if self.training:
-            # the reference's train() branch (pc_sam.py:150-165: mask-refinement iterations without new prompts, random
-            # prompt sampler, autograd) is not part of this inference-only path; fail instead of silently doing eval
-            raise NotImplementedError("psam_b200 is an inference-only path: call model.eval() (training mode of "
-                                      "PointCloudSAM.forward is not implemented)")
+            self._check_trainable()  # before any device work
         coords = coords if coords is not None else xyz
         features = features if features is not None else rgb
         gt_masks = gt_masks if gt_masks is not None else mask
         if gt_masks.dim() == 2:
             gt_masks = gt_masks.unsqueeze(1)
         gt_masks = gt_masks.bool()
+        if self.training:
+            return self._train_loop(coords.float().contiguous(), features.float().contiguous(), gt_masks, is_eval)
         enc = self._encode(coords.float().contiguous(), features.float().contiguous())
         return self._eval_loop(enc, coords, gt_masks, is_eval)
+
+    def _check_trainable(self):
+        """Training mode fine-tunes mask_decoder on a frozen encoder: every other parameter must have requires_grad=False.
+        A block with active dropout or drop-path is refused by the engine's block validation (the frozen encoder runs
+        deterministically, as in eval mode)."""
+        for name, p in self.named_parameters():
+            if p.requires_grad and not name.startswith("mask_decoder."):
+                raise NotImplementedError(
+                    f"training mode fine-tunes mask_decoder only, but parameter '{name}' has requires_grad=True: freeze "
+                    "everything else first with model.requires_grad_(False); model.mask_decoder.requires_grad_(True)")
+        engine.validate_transformer(self.pc_encoder.transformer)
+
+    def _train_loop(self, coords, features, gt_masks, is_eval):
+        """The reference's training forward (pc_sam.py:112-196) with only mask_decoder differentiable: the encoder, the
+        point and mask prompt encoders run through the engine as in eval mode, the decoder through psam_b200.train.  Two
+        iterations refine the mask without a new prompt (the last one and one drawn with torch.randint on the global CPU
+        generator, as in the reference); the fed-back mask reaches the mask encoder detached."""
+        from psam_b200 import train
+
+        B, M = coords.shape[0], gt_masks.shape[1]
+        refine = []
+        if self.enable_mask_refinement_iterations:
+            refine = [self.prompt_iters - 1]
+            if self.prompt_iters > 1:
+                refine.append(torch.randint(1, self.prompt_iters, (1,)).item())
+        with torch.no_grad():
+            enc = self._encode(coords, features)
+        patches = enc["patches"]
+        outputs = []
+        pc = coords.new_empty((B * M, 0, 3))
+        pl = gt_masks.new_empty((B * M, 0))
+        pm = None
+        for i in range(self.prompt_iters):
+            if i == 0 or i not in refine:
+                npc, npl = self._sample_prompts(coords, gt_masks, pm, is_eval)
+                pc = torch.cat([pc, npc], dim=1)
+                pl = torch.cat([pl, npl], dim=1)
+            with torch.no_grad():
+                sparse = engine.run_point_encoder(self.point_encoder, pc, pl, check=False)
+                dense = self.mask_encoder(None if pm is None else pm.detach(), coords, patches["centers"], patches["knn_idx"],
+                                          center_idx=self._center_idx(enc))
+            masks, iou = train.run_mask_decoder_train(self.mask_decoder, enc["pc_embeddings"], enc["pc_pe"], sparse, dense,
+                                                      enc["aux"], multimask_output=(i == 0))
+            engine.raise_if_out_of_range(masks.device)
+            if i == 0:
+                best = torch.argmax(iou.detach(), dim=1)
+                pm = batch_index_select(masks, best, dim=1)
+            else:
+                best = 0
+                pm = masks[:, 0]
+            outputs.append(dict(prompt_coords=pc, prompt_labels=pl, masks=masks, iou_preds=iou, max_iou_pred_ind=best,
+                                prompt_masks=pm))
+        return outputs
 
     def _eval_loop(self, enc, coords, gt_masks, is_eval, lengths=None):
         """The body of forward after the encode: `prompt_iters` rounds of prompt sampling from the ground truth
@@ -343,6 +396,10 @@ class PointCloudSAMHier(PointCloudSAM):
 
     def _center_idx(self, enc):
         return None  # MaskEncoderHier has no centralize_features
+
+    def _check_trainable(self):
+        raise NotImplementedError("training mode of PointCloudSAMHier is not implemented (fine-tuning covers PointCloudSAM's "
+                                  "MaskDecoder): call model.eval()")
 
     def _group_shape(self) -> tuple:
         pe = self.pc_encoder.patch_embed

@@ -958,11 +958,36 @@ def _decoder_heads(pk, queries, f0, aux, Z, T, G, D, rep, ids, mask_slice, dev):
     if aux.interp_index is None or aux.interp_weight is None:
         aux.interp_index, aux.interp_weight = ops.knn3_interp(aux.coords.float().contiguous(), aux.centers)
     N = aux.coords.shape[1]
-    u1 = Split(Z * N, D, dev)
-    nv.check(nv.lib().psam_interp_ln_gelu(nv.ptr(f0), Z, rep, G, D, nv.ptr(aux.interp_index), nv.ptr(aux.interp_weight), N,
-                                          nv.ptr(pk.up1[0]), nv.ptr(pk.up1[1]), pk.up1[2], u1.ptr(), u1.plane, u1.pitch,
-                                          nv.stream()), "interp_ln_gelu")
+    u1 = upscale_ln_gelu(f0, Z, rep, G, D, aux.interp_index, aux.interp_weight, N, pk.up1)
     return _mask_heads(pk, hs, u1, Z, T, N, D, ids, mask_slice, dev)
+
+
+def upscale_ln_gelu(f0, Z, rep, G, D, interp_index, interp_weight, N, up1) -> Split:
+    """output_upscaling[1..2] after the 3-NN interpolation of f0 = output_upscaling[0](keys) [Z*G, D] (the Linear commutes with
+    the interpolation): GELU(LayerNorm(interp(f0))) as split-bf16 [Z*N, D]; up1 = (gamma, beta, eps).  Shared by inference and
+    the fine-tuning head (psam_b200.train)."""
+    u1 = Split(Z * N, D, f0.device)
+    nv.check(nv.lib().psam_interp_ln_gelu(nv.ptr(f0), Z, rep, G, D, nv.ptr(interp_index), nv.ptr(interp_weight), N,
+                                          nv.ptr(up1[0]), nv.ptr(up1[1]), up1[2], u1.ptr(), u1.plane, u1.pitch,
+                                          nv.stream()), "interp_ln_gelu")
+    return u1
+
+
+def mask_product(u1: Split, up3w: Split, up3b, hyper, Z: int, C: int, N: int):
+    """masks [Z,C,N] = hyper [Z,C,Du] . GELU(u1 @ up3w^T + up3b) (output_upscaling[3..4] and mask_decoder.py:176).  Shared by
+    inference and the fine-tuning head (psam_b200.train)."""
+    dev = hyper.device
+    Du = up3w.rows
+    if FUSED_MASK_DOT and N % 32 == 0 and C <= 8:
+        # output_upscaling[3..4] (Linear + GELU) and the hyper-network product fused into one GEMM epilogue
+        masks = torch.zeros((Z, C, N), dtype=torch.float32, device=dev)
+        ops.gemm(u1, up3w, bias=up3b, act=ACT_GELU, passes=PASSES, rowdot=(hyper, masks))
+    else:
+        u2 = torch.empty((Z * N, Du), dtype=torch.float32, device=dev)
+        ops.gemm(u1, up3w, bias=up3b, out_f32=u2, act=ACT_GELU, passes=PASSES)
+        masks = torch.empty((Z, C, N), dtype=torch.float32, device=dev)
+        nv.check(nv.lib().psam_mask_dot(nv.ptr(u2), Du, nv.ptr(hyper), Z, C, N, Du, nv.ptr(masks), nv.stream()), "mask_dot")
+    return masks
 
 
 def _mask_heads(pk, hs, u1, Z, T, N, D, ids, mask_slice, dev):
@@ -981,16 +1006,7 @@ def _mask_heads(pk, hs, u1, Z, T, N, D, ids, mask_slice, dev):
         ops.linear_f32(x, w[i0:i0 + C], b[i0:i0 + C], act=ACT_RELU if li < 2 else ACT_NONE, out=y, M=Z, K=Ki, ldx=ld, Z=C,
                        x_z=Ki, w_z=Do * Ki, b_z=Do, y_z=Do, ldy=C * Do, x_off=xoff)
         x, ld, xoff, hyper = y, C * Do, 0, y
-    Du = pk.up3w.rows
-    if FUSED_MASK_DOT and N % 32 == 0 and C <= 8:
-        # output_upscaling[3..4] (Linear + GELU) and the hyper-network product fused into one GEMM epilogue
-        masks = torch.zeros((Z, C, N), dtype=torch.float32, device=dev)
-        ops.gemm(u1, pk.up3w, bias=pk.up3b, act=ACT_GELU, passes=PASSES, rowdot=(hyper, masks))
-    else:
-        u2 = torch.empty((Z * N, Du), dtype=torch.float32, device=dev)
-        ops.gemm(u1, pk.up3w, bias=pk.up3b, out_f32=u2, act=ACT_GELU, passes=PASSES)
-        masks = torch.empty((Z, C, N), dtype=torch.float32, device=dev)
-        nv.check(nv.lib().psam_mask_dot(nv.ptr(u2), Du, nv.ptr(hyper), Z, C, N, Du, nv.ptr(masks), nv.stream()), "mask_dot")
+    masks = mask_product(u1, pk.up3w, pk.up3b, hyper, Z, C, N)
 
     # IoU head on the iou token (mask_decoder.py:180-182)
     y = hs
@@ -1042,8 +1058,5 @@ def _decoder_heads_hier(pk, queries, f2, aux, Z, T, G2, D, rep, ids, mask_slice,
     Dh = pk.mid_w.rows
     f1 = torch.empty((Z * G1, Dh), dtype=torch.float32, device=dev)
     ops.gemm(h, pk.mid_w, bias=pk.mid_b, out_f32=f1, passes=PASSES)
-    u1 = Split(Z * N, Dh, dev)
-    nv.check(nv.lib().psam_interp_ln_gelu(nv.ptr(f1), Z, rep, G1, Dh, nv.ptr(aux1.interp_index), nv.ptr(aux1.interp_weight), N,
-                                          nv.ptr(pk.up1[0]), nv.ptr(pk.up1[1]), pk.up1[2], u1.ptr(), u1.plane, u1.pitch,
-                                          nv.stream()), "interp_ln_gelu")
+    u1 = upscale_ln_gelu(f1, Z, rep, G1, Dh, aux1.interp_index, aux1.interp_weight, N, pk.up1)
     return _mask_heads(pk, queries, u1, Z, T, N, D, ids, mask_slice, dev)

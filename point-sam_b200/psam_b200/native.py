@@ -72,6 +72,8 @@ EXPORTS = [
     "psam_crop_edge_filter_batched", "psam_crop_run_bytes", "psam_crop_uncrop_batched",
     "psam_mesh_sample_workspace_bytes", "psam_mesh_sample_f32", "psam_mesh_face_centers_f32", "psam_mask_lift", "psam_mask_label_map",
     "psam_nn_grid_workspace_bytes", "psam_nn_grid_f32", "psam_voxel_subsample_workspace_bytes", "psam_voxel_subsample_f32",
+    "psam_mask_loss_stats", "psam_mask_loss_grad", "psam_interp_inverse", "psam_head_dp", "psam_head_dp_chunks",
+    "psam_interp_ln_gelu_backward", "psam_interp_backward", "psam_sum_partials",
     "psam_version",
 ]
 
@@ -110,6 +112,8 @@ def lib():
         L.psam_nn_grid_workspace_bytes.argtypes = [i]
         L.psam_voxel_subsample_workspace_bytes.restype = c_size_t
         L.psam_voxel_subsample_workspace_bytes.argtypes = [i]
+        L.psam_head_dp_chunks.restype = c_int
+        L.psam_head_dp_chunks.argtypes = [i]
         sig = {
             "psam_fps_f32": [p, i, i, i, p, p, p, p],
             "psam_knn_f32": [p, p, i, i, i, i, p, p, p],
@@ -165,6 +169,13 @@ def lib():
             "psam_mask_label_map": [p, i, i, p, i, p, p],
             "psam_nn_grid_f32": [p, i, p, i, p, p, p, p],
             "psam_voxel_subsample_f32": [p, i, i, ctypes.c_uint64, p, p, p, p],
+            "psam_mask_loss_stats": [p, p, i, i, i, p, p, p],
+            "psam_mask_loss_grad": [p, p, i, i, i, p, p, p, p],
+            "psam_interp_inverse": [p, i, i, i, p, p, p],
+            "psam_head_dp": [p, p, p, i, i, i, i, p, ll, ll, p, p, p],
+            "psam_interp_ln_gelu_backward": [p, i, i, i, i, p, p, i, p, p, f, p, p, i, p],
+            "psam_interp_backward": [p, i, i, i, i, p, p, p, i, p, p],
+            "psam_sum_partials": [p, i, i, ll, p, p],
         }
         for name, args in sig.items():
             fn = getattr(L, name)
