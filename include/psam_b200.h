@@ -337,7 +337,8 @@ int psam_decoder_prepare(const float* iou_token, const float* mask_tokens, int n
 
 /* 3-NN feature upsampling fused with LayerNorm + GELU: y[z*N+n,:] = GELU(LN(sum_k w[b,n,k]*f[z,idx[b,n,k],:])),
  * b = z/rep; split-bf16 output.  Replaces interpolate_features (common.py:258-274) + output_upscaling[1..2]
- * (mask_decoder.py:55-56) after output_upscaling[0] has been applied to the patch features. */
+ * (mask_decoder.py:55-56) after output_upscaling[0] has been applied to the patch features.  D in {128, 256, 512, 1024}
+ * (PSAM_ERR_UNSUPPORTED otherwise, as for psam_interp_add_ln_gelu). */
 int psam_interp_ln_gelu(const float* f, int Z, int rep, int G, int D, const long long* idx, const float* w, int N,
                         const float* gamma, const float* beta, float eps, void* y_hi, long long y_plane,
                         long long ldy_s, cudaStream_t stream);
@@ -729,14 +730,16 @@ int psam_mask_loss_stats(const float* logits, const unsigned char* gt, int Z, in
 
 /* dlogits[z,c,n] = dloss[z,c] * d(focal_mean + 2 dice)[z,c] / dlogit[z,c,n], dice = 1 - (2 sum p t + 1e-3) / (sum p^2 + sum t
  * + 1e-3), from psam_mask_loss_stats' stats.  A (z, c) with dloss == 0 (a mask the criterion did not select) is written as
- * zeros without evaluating its terms.  Z * C <= 65535.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+ * +0.0 (also for dloss == -0.0) without evaluating its terms, so NaN or infinite logits in such a row do not reach dlogits.
+ * Z * C <= 65535.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
 int psam_mask_loss_grad(const float* logits, const unsigned char* gt, int Z, int C, int N, const float* stats, const float* dloss,
                         float* dlogits, cudaStream_t stream);
 
 /* Inverse of the 3-NN interpolation index idx [B,N,3] (int64, values in [0, G); psam_knn3_interp_f32): per cloud b,
  * offsets[b, g] .. offsets[b, g+1] (int32 [B, G+1]) delimit the entries e = n * 3 + k with idx[b,n,k] == g in entries
- * (int32 [B, 3N]), in ascending e.  One CTA per cloud; a stable counting sort.  G <= 8192.  Bad arguments -> PSAM_ERR_ARG
- * before any CUDA call. */
+ * (int32 [B, 3N]), in ascending e; offsets[b, 0] = 0 and offsets[b, G] = 3N.  One CTA per cloud; a stable counting sort.
+ * G <= 8192.  Every index must lie in [0, G): an entry outside it is skipped (neither counted nor placed), so offsets[b, G]
+ * falls short of 3N and the tail of entries[b] is left unwritten.  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
 int psam_interp_inverse(const long long* idx, int B, int N, int G, int* offsets, int* entries, cudaStream_t stream);
 
 /* Head backward, elementwise part.  p [Z*N, D] = output_upscaling[3] pre-activation (fp32), dm [Z,C,N] the gradient of the
@@ -758,8 +761,10 @@ int psam_interp_ln_gelu_backward(const float* f, int Z, int rep, int G, int D, c
                                  cudaStream_t stream);
 
 /* Backward of the 3-NN interpolation (interpolate_features, common.py:258-274) as a gather: df[z*G+g, :] = sum over the
- * entries e of patch g of cloud b = z / rep (psam_interp_inverse, in its order) of w[b, e] * dv[z*N + e/3, :].  D a multiple of
- * 128 <= 1024 (PSAM_ERR_UNSUPPORTED otherwise).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
+ * entries e of patch g of cloud b = z / rep (psam_interp_inverse, in its order) of w[b, e] * dv[z*N + e/3, :], one fp32 fma
+ * per entry in that order.
+ * D in {128, 256, 512, 1024} (PSAM_ERR_UNSUPPORTED otherwise).  A patch with no entries gets rows of +0.0.  Bad arguments ->
+ * PSAM_ERR_ARG before any CUDA call. */
 int psam_interp_backward(const float* dv, int Z, int rep, int G, int D, const int* offsets, const int* entries, const float* w, int N,
                          float* df, cudaStream_t stream);
 

@@ -294,6 +294,9 @@ class PointCloudSAM(nn.Module):
                 raise NotImplementedError(
                     f"training mode fine-tunes mask_decoder only, but parameter '{name}' has requires_grad=True: freeze "
                     "everything else first with model.requires_grad_(False); model.mask_decoder.requires_grad_(True)")
+        from psam_b200 import train
+
+        train.check_head_shape(self.mask_decoder.transformer_dim, self._group_shape()[0])
         engine.validate_transformer(self.pc_encoder.transformer)
 
     def _train_loop(self, coords, features, gt_masks, is_eval):

@@ -31,6 +31,20 @@ BACKWARD_ROWS = 262144
 # K rows of each partial product of the weight gradient dW3 = dp^T u1 (fixed partial buffers, summed in a fixed order)
 DW_SPLIT_K = 4096
 LN_ROWS_PER_BLOCK = 256
+# decoder widths of psam_interp_ln_gelu_backward, and the most patches psam_interp_inverse sorts in one CTA
+TRAIN_WIDTHS = (128, 256, 512)
+MAX_TRAIN_GROUPS = 8192
+
+
+def check_head_shape(D: int, G: int):
+    """Refuses a decoder width or patch count the head backward has no kernel for (NotImplementedError), so that training
+    stops before any device work rather than in loss.backward()."""
+    if D not in TRAIN_WIDTHS:
+        raise NotImplementedError(f"fine-tuning supports decoder widths {', '.join(map(str, TRAIN_WIDTHS))} (the LayerNorm "
+                                  f"backward of the mask head), got {D}")
+    if G > MAX_TRAIN_GROUPS:
+        raise NotImplementedError(f"fine-tuning supports at most {MAX_TRAIN_GROUPS} patches per cloud (the inverse of the "
+                                  f"interpolation index), got {G}")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -299,6 +313,7 @@ def run_mask_decoder_train(md, pc_embeddings, pc_pe, sparse, dense, aux, multima
         raise NotImplementedError("fine-tuning covers MaskDecoder; the backward of MaskDecoderHier is not implemented")
     Z = sparse.shape[0]
     B, G, _ = pc_embeddings.shape
+    check_head_shape(md.transformer_dim, G)
     f0, hyper, iou_pred = decoder_trunk(md, pc_embeddings, pc_pe, sparse, dense, multimask_output)
     up = md.output_upscaling
     geo = head_geometry(aux, G, Z // B, up[1].eps)

@@ -67,6 +67,29 @@ def test_training_refuses_an_active_drop_path():
         m(*_inputs())
 
 
+def test_training_refuses_a_width_or_patch_count_without_a_backward_before_any_device_work():
+    """Inference takes decoder widths 128, 256, 512 and 1024, but the head backward has LayerNorm kernels for 128, 256 and
+    512 only, and sorts at most 8192 patches per cloud: training refuses the rest up front, naming what it supports (a CPU
+    model: the refusal comes before the engine's CUDA-only error)."""
+    from pc_sam.model import build_point_sam
+
+    for D in (384, 1024):
+        m = build_point_sam("eva02_test_tiny", 8, 4, embed_dim=D).train()
+        m.requires_grad_(False)
+        m.mask_decoder.requires_grad_(True)
+        with pytest.raises(NotImplementedError, match=rf"decoder widths 128, 256, 512.*got {D}"):
+            m(*_inputs())
+    m = build_point_sam("eva02_test_tiny", 8193, 4).train()
+    m.requires_grad_(False)
+    m.mask_decoder.requires_grad_(True)
+    with pytest.raises(NotImplementedError, match=r"at most 8192 patches.*got 8193"):
+        m(*_inputs())
+    m = build_point_sam("eva02_test_tiny", 8, 4, embed_dim=128).train()  # a supported width passes the refusals
+    m.requires_grad_(False)
+    m.mask_decoder.requires_grad_(True)
+    m._check_trainable()
+
+
 @pytest.fixture(scope="module")
 def lib():
     from psam_b200 import build
@@ -79,20 +102,28 @@ def test_finetune_entry_points_validate_arguments_without_gpu(lib):
     P = ctypes.c_void_p(16)  # never dereferenced: validation fails first
     f = ctypes.c_float(1e-5)
     for fn in ("psam_mask_loss_stats", "psam_mask_loss_grad", "psam_interp_inverse", "psam_head_dp", "psam_interp_ln_gelu_backward",
-               "psam_interp_backward", "psam_sum_partials"):
+               "psam_interp_backward", "psam_sum_partials", "psam_interp_ln_gelu"):
         getattr(lib, fn).restype = ctypes.c_int
     assert lib.psam_mask_loss_stats(None, P, 1, 1, 8, P, P, None) == -1
     assert lib.psam_mask_loss_stats(P, P, 1, 0, 8, P, P, None) == -1
+    assert lib.psam_mask_loss_stats(P, P, 65536, 32768, 8, P, P, None) == -1  # Z * C = 2^31 > 2^31 - 1
     assert lib.psam_mask_loss_grad(P, P, 1, 1, 8, P, None, P, None) == -1
     assert lib.psam_mask_loss_grad(P, P, 256, 256, 8, P, P, P, None) == -1  # Z * C > 65535
     assert lib.psam_interp_inverse(P, 1, 8, 0, P, P, None) == -1
     assert lib.psam_interp_inverse(P, 1, 8, 8193, P, P, None) == -1
     assert lib.psam_head_dp(P, P, P, 1, 9, 8, 256, P, ctypes.c_longlong(0), ctypes.c_longlong(256), P, P, None) == -1  # C > 8
     assert lib.psam_head_dp(P, P, P, 1, 3, 8, 250, P, ctypes.c_longlong(0), ctypes.c_longlong(256), P, P, None) == -1  # D % 32
+    assert lib.psam_head_dp(P, P, P, 1, 3, 8, 1056, P, ctypes.c_longlong(0), ctypes.c_longlong(1056), P, P, None) == -1  # D > 1024
+    assert lib.psam_head_dp(P, P, P, 1, 3, 8, 256, P, ctypes.c_longlong(0), ctypes.c_longlong(224), P, P, None) == -1  # ldp_s < D
     assert lib.psam_interp_ln_gelu_backward(P, 1, 1, 4, 256, P, P, 8, P, P, f, None, P, 256, None) == -1
     assert lib.psam_interp_ln_gelu_backward(P, 1, 1, 4, 1024, P, P, 8, P, P, f, P, P, 256, None) == -2  # D > 512
     assert lib.psam_interp_backward(P, 1, 1, 4, 256, None, P, P, 8, P, None) == -1
     assert lib.psam_interp_backward(P, 1, 1, 4, 200, P, P, P, 8, P, None) == -2
+    # the interpolation forward and backward have kernels for D in {128, 256, 512, 1024}, not every multiple of 128
+    for D in (384, 640, 768, 896, 1152):
+        assert lib.psam_interp_backward(P, 1, 1, 4, D, P, P, P, 8, P, None) == -2, D
+        assert lib.psam_interp_ln_gelu(P, 1, 1, 4, D, P, P, 8, P, P, f, P, ctypes.c_longlong(0), ctypes.c_longlong(D), None) == -2, D
+    assert lib.psam_interp_ln_gelu_backward(P, 1, 1, 4, 384, P, P, 8, P, P, f, P, P, 256, None) == -2
     assert lib.psam_sum_partials(P, 1, 0, ctypes.c_longlong(4), P, None) == -1
     lib.psam_head_dp_chunks.restype = ctypes.c_int
     assert lib.psam_head_dp_chunks(32768) == 256 and lib.psam_head_dp_chunks(1) == 1
