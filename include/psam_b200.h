@@ -772,6 +772,41 @@ int psam_interp_backward(const float* dv, int Z, int rep, int G, int D, const in
  * every partial-sum buffer above (and of split-K GEMM partials).  Bad arguments -> PSAM_ERR_ARG before any CUDA call. */
 int psam_sum_partials(const float* part, int nb, int S, long long n, float* out, cudaStream_t stream);
 
+/* Encoder fine-tuning (csrc/train_encoder.cu): the row-wise steps of a timm EvaBlock's backward; its matrix products run on
+ * psam_gemm_bf16x3.  Every width has a kernel (rows are walked by a warp in steps of 32 columns).  No atomics: the outputs
+ * are a fixed-order function of the inputs.  Bad arguments -> PSAM_ERR_ARG before any CUDA call.
+ *
+ * LayerNorm backward over rows x [M, ldx] of D columns with dL/dy dy [M, ldy] and the weight gamma [D] (mean and variance
+ * recomputed with the forward's two-pass arithmetic): dx [M, ldo] = the gradient with respect to x, plus dres [M, ldr] when
+ * it is not NULL (the residual branch's gradient); dx_hi (nullable) receives the same values as split-bf16 (lo plane dx_plane
+ * elements after the hi plane, row stride dx_ld).  part [ceil(M / rows_per_block), 2, D]: per block of rows_per_block
+ * consecutive rows, the sums of dy x_hat (-> dgamma) and of dy (-> dbeta) in row order; psam_sum_partials finishes them.
+ * 1 <= rows_per_block <= 1024. */
+int psam_layernorm_backward(const float* x, long long ldx, int M, int D, const float* dy, long long ldy, const float* gamma, float eps,
+                            const float* dres, long long ldr, float* dx, long long ldo, void* dx_hi, long long dx_plane, long long dx_ld,
+                            float* part, int rows_per_block, cudaStream_t stream);
+
+/* SwiGLU with its inner LayerNorm (timm SwiGLU, scale_mlp=True), backward from dL/d LN(h) dhn [M, ldd] (Hd columns) to the
+ * interleaved pre-activation a [M, lda] = [g_0 x_0 g_1 x_1 ...] of the fc1 GEMM (2 Hp columns, h_i = silu(g_i) x_i for
+ * i < Hd, zero padding up to Hp).  da [M, ldo] = d[g | x] in the same interleaved layout, columns 2 Hd .. 2 Hp written as 0;
+ * da_hi (nullable) the same as split-bf16.  hn_hi (nullable) receives LN(h) = x_hat gamma + beta as split-bf16 [M, Hp] with
+ * zero padding (the operand of fc2's weight gradient).  part [ceil(M / rows_per_block), 2, Hd] as psam_layernorm_backward.
+ * lda and ldo even, 1 <= rows_per_block <= 1024. */
+int psam_swiglu_ln_backward(const float* a, long long lda, int M, int Hd, int Hp, const float* dhn, long long ldd, const float* gamma,
+                            const float* beta, float eps, float* da, long long ldo, void* da_hi, long long da_plane, long long da_ld,
+                            void* hn_hi, long long hn_plane, long long hn_ld, float* part, int rows_per_block, cudaStream_t stream);
+
+/* GELU backward over a [M, lda] (n columns): da = dh * GELU'(a) with the exact-erf derivative Phi(a) + a phi(a), to da
+ * [M, ldo] and / or da_hi (split-bf16); h_hi (nullable) receives GELU(a) with the forward's arithmetic (the A&S erf of the
+ * GEMM epilogue) as split-bf16.  At least one output. */
+int psam_gelu_backward(const float* a, long long lda, int M, int n, const float* dh, long long ldd, float* da, long long ldo, void* da_hi,
+                       long long da_plane, long long da_ld, void* h_hi, long long h_plane, long long h_ld, cudaStream_t stream);
+
+/* Softmax backward over rows of L raw scores s [rows, lds] with P = softmax(scale s) recomputed as psam_softmax_split does:
+ * dS = scale P (dP - sum_j dP_j P_j) as split-bf16 [rows, ds_ld] (the gradient with respect to the raw scores). */
+int psam_softmax_backward(const float* s, long long lds, const float* dp, long long lddp, long long rows, int L, float scale, void* ds_hi,
+                          long long ds_plane, long long ds_ld, cudaStream_t stream);
+
 const char* psam_version(void);
 
 #ifdef __cplusplus

@@ -2,7 +2,7 @@
 ``set_pointcloud`` / 4-argument ``predict_masks`` form that demo/app.py:198-205 calls.
 
 All computation runs in the sm_90a kernels behind ``psam_b200`` (no CPU / PyTorch fallback).  Training mode fine-tunes
-mask_decoder on a frozen encoder (psam_b200.train); everything else is inference."""
+mask_decoder and, optionally, the encoder's transformer (psam_b200.train); everything else is inference."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -41,6 +41,9 @@ class PointCloudSAM(nn.Module):
         """lengths [B] int32 (device): coords / features are padded clouds (ops.pad_clouds), cloud b its first lengths[b]
         points; the caller has checked every lengths[b] >= the first-level num_groups (varlen_clouds)."""
         pc_embeddings, patches = self._run_encoder(coords, features, lengths)
+        return self._encoded(pc_embeddings, patches, coords, features)
+
+    def _encoded(self, pc_embeddings, patches, coords, features):
         centers = patches["centers"]
         aux = AuxInputs(coords=coords, features=features, centers=centers)
         pc_pe = engine.run_pos_embedding(self.point_encoder.pe_layer, centers, check=False)
@@ -286,22 +289,32 @@ class PointCloudSAM(nn.Module):
         return self._eval_loop(enc, coords, gt_masks, is_eval)
 
     def _check_trainable(self):
-        """Training mode fine-tunes mask_decoder on a frozen encoder: every other parameter must have requires_grad=False.
-        A block with active dropout or drop-path is refused by the engine's block validation (the frozen encoder runs
-        deterministically, as in eval mode)."""
-        for name, p in self.named_parameters():
-            if p.requires_grad and not name.startswith("mask_decoder."):
-                raise NotImplementedError(
-                    f"training mode fine-tunes mask_decoder only, but parameter '{name}' has requires_grad=True: freeze "
-                    "everything else first with model.requires_grad_(False); model.mask_decoder.requires_grad_(True)")
+        """Training mode fine-tunes mask_decoder and the point-cloud encoder after its tokenizer: the transformer blocks,
+        the tail LayerNorms, out_proj, patch_proj and pos_embed, in any combination.  Every other parameter (the tokenizer,
+        point_encoder, mask_encoder) must have requires_grad=False; the first one that does not is named.  A block with
+        active dropout or drop-path is refused by the engine's block validation (the encoder runs deterministically, as in
+        eval mode), and so is a trainable block without a backward kernel."""
         from psam_b200 import train
 
+        enc_ok = tuple("pc_encoder." + p for p in train.ENCODER_TRAINABLE)
+        for name, p in self.named_parameters():
+            if p.requires_grad and not name.startswith(("mask_decoder.",) + enc_ok):
+                raise NotImplementedError(
+                    f"training mode fine-tunes mask_decoder and pc_encoder's transformer blocks, norm / fc_norm, out_proj, "
+                    f"patch_proj and pos_embed, but parameter '{name}' has requires_grad=True: freeze everything else first "
+                    "with model.requires_grad_(False); model.mask_decoder.requires_grad_(True) (and, to adapt the encoder, "
+                    "e.g. model.pc_encoder.transformer.blocks[-4:].requires_grad_(True))")
         train.check_head_shape(self.mask_decoder.transformer_dim, self._group_shape()[0])
         engine.validate_transformer(self.pc_encoder.transformer)
+        D = self.pc_encoder.transformer_dim
+        for blk in self.pc_encoder.transformer.blocks:
+            if any(p.requires_grad for p in blk.parameters()):
+                train.check_block_shape(blk, D)
 
     def _train_loop(self, coords, features, gt_masks, is_eval):
-        """The reference's training forward (pc_sam.py:112-196) with only mask_decoder differentiable: the encoder, the
-        point and mask prompt encoders run through the engine as in eval mode, the decoder through psam_b200.train.  Two
+        """The reference's training forward (pc_sam.py:112-196) with mask_decoder and the encoder's trainable parameters
+        differentiable: the point and mask prompt encoders run through the engine as in eval mode, the decoder through
+        psam_b200.train, and the encoder too when any of its parameters trains (without gradient otherwise).  Two
         iterations refine the mask without a new prompt (the last one and one drawn with torch.randint on the global CPU
         generator, as in the reference); the fed-back mask reaches the mask encoder detached."""
         from psam_b200 import train
@@ -312,8 +325,13 @@ class PointCloudSAM(nn.Module):
             refine = [self.prompt_iters - 1]
             if self.prompt_iters > 1:
                 refine.append(torch.randint(1, self.prompt_iters, (1,)).item())
-        with torch.no_grad():
-            enc = self._encode(coords, features)
+        if train.encoder_trains(self.pc_encoder):
+            pc_embeddings, patches = train.run_pc_encoder_train(self.pc_encoder, coords, features)
+            with torch.no_grad():
+                enc = self._encoded(pc_embeddings, patches, coords, features)
+        else:
+            with torch.no_grad():
+                enc = self._encode(coords, features)
         patches = enc["patches"]
         outputs = []
         pc = coords.new_empty((B * M, 0, 3))

@@ -73,8 +73,10 @@ def _fingerprint(module) -> tuple:
         (b.data_ptr(), b._version) for b in module.buffers())
 
 
-def _cached(module, builder):
-    fp = _fingerprint(module)
+def _cached(module, builder, key=()):
+    """builder(module), cached on the module until a parameter or buffer changes (or `key`, for packs that depend on
+    module-level switches)."""
+    fp = (_fingerprint(module), key)
     c = module.__dict__.get("_psam_packed")
     if c is None or c[0] != fp:
         if any(not p.is_cuda for p in module.parameters()):
@@ -410,30 +412,59 @@ def _fold_ln(w: torch.Tensor, b: torch.Tensor, norm):
     return ops.pack_weight(wg.float()), wg.sum(dim=1).float().contiguous(), (wd @ be + b.detach().double()).float().contiguous()
 
 
+def qkv_weights(at, D: int):
+    """(W [3D, D], b [3D]) fp32 of q / k / v stacked, from a fused qkv (q_bias, zero k, v_bias) or from q_proj / k_proj /
+    v_proj."""
+    zeros = torch.zeros(D, dtype=torch.float32, device=at.proj.weight.device)
+    if getattr(at, "qkv", None) is not None:
+        wqkv = at.qkv.weight.detach().float()
+        qb = at.q_bias.detach().float() if getattr(at, "q_bias", None) is not None else zeros
+        vb = at.v_bias.detach().float() if getattr(at, "v_bias", None) is not None else zeros
+        return wqkv, torch.cat([qb, zeros, vb]).contiguous()
+    wqkv = torch.cat([at.q_proj.weight, at.k_proj.weight, at.v_proj.weight]).detach().float()
+    bias = lambda lin: lin.bias.detach().float() if lin.bias is not None else zeros
+    return wqkv, torch.cat([bias(at.q_proj), bias(at.k_proj), bias(at.v_proj)]).contiguous()
+
+
+def swiglu_hidden_pad(Hd: int) -> int:
+    return (Hd + 63) // 64 * 64
+
+
+def swiglu_fc1(mlp, Hp: int):
+    """(W1 [2 Hp, D], b1 [2 Hp]) fp32: fc1_g / fc1_x rows interleaved (2i, 2i+1), zero rows from 2 Hd on."""
+    Hd, D = mlp.fc1_g.out_features, mlp.fc1_g.in_features
+    dev = mlp.fc1_g.weight.device
+    w1 = torch.zeros((2 * Hp, D), dtype=torch.float32, device=dev)
+    b1 = torch.zeros(2 * Hp, dtype=torch.float32, device=dev)
+    w1[0:2 * Hd:2], w1[1:2 * Hd:2] = mlp.fc1_g.weight.detach().float(), mlp.fc1_x.weight.detach().float()
+    b1[0:2 * Hd:2], b1[1:2 * Hd:2] = mlp.fc1_g.bias.detach().float(), mlp.fc1_x.bias.detach().float()
+    return w1, b1
+
+
+def swiglu_fc2(mlp, Hp: int):
+    """fc2's weight [D, Hp] fp32, zero columns from Hd on."""
+    w2 = torch.zeros((mlp.fc2.out_features, Hp), dtype=torch.float32, device=mlp.fc2.weight.device)
+    w2[:, :mlp.fc2.in_features] = mlp.fc2.weight.detach().float()
+    return w2
+
+
 class _PackedBlock:
     def __init__(self, blk, D):
         validate_eva_block(blk)
         at = blk.attn
-        self.H, self.dh = at.num_heads, D // at.num_heads
+        self.D, self.H, self.dh = D, at.num_heads, D // at.num_heads
         self.g1, self.b1, self.eps1 = _f32(blk.norm1.weight), _f32(blk.norm1.bias), blk.norm1.eps
         self.g2, self.b2, self.eps2 = _f32(blk.norm2.weight), _f32(blk.norm2.bias), blk.norm2.eps
         dev = blk.norm1.weight.device
-        zeros = torch.zeros(D, dtype=torch.float32, device=dev)
-        if getattr(at, "qkv", None) is not None:
-            wqkv = at.qkv.weight.detach().float()
-            qb = at.q_bias.detach().float() if getattr(at, "q_bias", None) is not None else zeros
-            vb = at.v_bias.detach().float() if getattr(at, "v_bias", None) is not None else zeros
-            bqkv = torch.cat([qb, zeros, vb])
-        else:
-            wqkv = torch.cat([at.q_proj.weight, at.k_proj.weight, at.v_proj.weight]).detach().float()
-            bias = lambda lin: lin.bias.detach().float() if lin.bias is not None else zeros
-            bqkv = torch.cat([bias(at.q_proj), bias(at.k_proj), bias(at.v_proj)])
-        self.wqkv, self.bqkv = ops.pack_weight(wqkv), bqkv.contiguous()
+        wqkv, bqkv = qkv_weights(at, D)
+        self.wqkv, self.bqkv = ops.pack_weight(wqkv), bqkv
+        self.transposed = None  # the W^T operands of the backward (psam_b200.train), packed on first use
         # the folded forms live in the GEMM's vectorised epilogue (whole 32-column chunks): D and the MLP width must be
-        # multiples of 32, otherwise the block keeps its LayerNorm kernels
+        # multiples of 32, otherwise the block keeps its LayerNorm kernels.  Whether the encoder uses them is decided for
+        # all blocks together (_PackedEncoder.fold_block).
         mlp_w = blk.mlp.fc1_g.out_features if hasattr(blk.mlp, "fc1_g") else blk.mlp.fc1.out_features
-        self.fold_block = FUSED_BLOCK_LN and D % 32 == 0 and (hasattr(blk.mlp, "fc1_g") or mlp_w % 32 == 0)
-        if self.fold_block:
+        self.can_fold = FUSED_BLOCK_LN and D % 32 == 0 and (hasattr(blk.mlp, "fc1_g") or mlp_w % 32 == 0)
+        if self.can_fold:
             # LN(x) @ W^T + b = rstd * (x @ (W gamma)^T - mean * (W gamma) 1) + (W beta + b)
             self.wqkv_f, self.cqkv, self.bqkv_f = _fold_ln(wqkv, bqkv, blk.norm1)
         self.wproj, self.bproj = ops.pack_weight(at.proj.weight), _f32(at.proj.bias)
@@ -441,22 +472,18 @@ class _PackedBlock:
         self.swiglu = hasattr(mlp, "fc1_g")
         if self.swiglu:
             Hd = mlp.fc1_g.out_features
-            Hp = (Hd + 63) // 64 * 64
-            w1 = torch.zeros((2 * Hp, D), dtype=torch.float32, device=dev)
-            b1 = torch.zeros(2 * Hp, dtype=torch.float32, device=dev)
+            Hp = swiglu_hidden_pad(Hd)
             # gate / value rows interleaved (2i, 2i+1): the GEMM epilogue computes silu(g) * x directly
-            w1[0:2 * Hd:2], w1[1:2 * Hd:2] = mlp.fc1_g.weight.detach().float(), mlp.fc1_x.weight.detach().float()
-            b1[0:2 * Hd:2], b1[1:2 * Hd:2] = mlp.fc1_g.bias.detach().float(), mlp.fc1_x.bias.detach().float()
+            w1, b1 = swiglu_fc1(mlp, Hp)
             self.hid, self.hp = Hd, Hp
             self.w1, self.bb1 = ops.pack_weight(w1), b1
-            if self.fold_block:
+            if self.can_fold:
                 self.w1_f, self.c1, self.bb1_f = _fold_ln(w1, b1, blk.norm2)
             gpad = torch.zeros(Hp, dtype=torch.float32, device=dev)
             bpad = torch.zeros(Hp, dtype=torch.float32, device=dev)
             gpad[:Hd], bpad[:Hd] = mlp.norm.weight.detach().float(), mlp.norm.bias.detach().float()
             self.gn, self.bn, self.epsn = gpad, bpad, mlp.norm.eps  # zero-padded to Hp for the float4 LN path
-            w2 = torch.zeros((D, Hp), dtype=torch.float32, device=dev)
-            w2[:, :Hd] = mlp.fc2.weight.detach().float()
+            w2 = swiglu_fc2(mlp, Hp)
             self.fold_ln = FUSED_INNER_LN
             if self.fold_ln:
                 # fc2(LN(h)) = rstd * (h @ (W2 * gamma)^T - mean * (W2 @ gamma)) + (W2 @ beta + b2): the normalisation becomes a
@@ -470,7 +497,7 @@ class _PackedBlock:
         else:
             self.hid = mlp.fc1.out_features
             self.w1, self.bb1 = ops.pack_weight(mlp.fc1.weight), _f32(mlp.fc1.bias)
-            if self.fold_block:
+            if self.can_fold:
                 self.w1_f, self.c1, self.bb1_f = _fold_ln(mlp.fc1.weight.detach().float(), mlp.fc1.bias.detach().float(), blk.norm2)
             self.w2, self.bb2 = ops.pack_weight(mlp.fc2.weight), _f32(mlp.fc2.bias)
 
@@ -483,16 +510,20 @@ class _PackedEncoder:
         self.wpos0, self.bpos0 = _f32(enc.pos_embed[0].weight), _f32(enc.pos_embed[0].bias)
         self.wpos2, self.bpos2 = ops.pack_weight(enc.pos_embed[2].weight), _f32(enc.pos_embed[2].bias)
         self.tail = [(_f32(m.weight), _f32(m.bias), m.eps) for m in validate_transformer(enc.transformer)]
-        self.blocks = [_PackedBlock(b, D) for b in enc.transformer.blocks]
+        self.blocks = [block_pack(b, D) for b in enc.transformer.blocks]
         self.wout, self.bout = ops.pack_weight(enc.out_proj.weight), _f32(enc.out_proj.bias)
-        self.fold_block = (FUSED_BLOCK_LN and len(self.tail) == 1 and all(b.fold_block for b in self.blocks)
+        self.fold_block = (FUSED_BLOCK_LN and len(self.tail) == 1 and all(b.can_fold for b in self.blocks)
                            and enc.embed_dim % 32 == 0)
-        for b in self.blocks:
-            b.fold_block = self.fold_block
         if self.fold_block:
             m = validate_transformer(enc.transformer)[0]
             self.wout_f, self.cout, self.bout_f = _fold_ln(enc.out_proj.weight.detach().float(), enc.out_proj.bias.detach().float(), m)
             self.eps_tail = m.eps
+
+
+def block_pack(blk, D: int) -> _PackedBlock:
+    """The packed weights of one EvaBlock, cached on the block: after an optimizer step only the blocks whose parameters
+    changed are packed again."""
+    return _cached(blk, lambda m: _PackedBlock(m, D), key=(FUSED_BLOCK_LN, FUSED_INNER_LN))
 
 
 def _attention_unfused(qkv: Split, att: Split, B: int, L: int, H: int, dh: int, D: int, dev):
@@ -522,6 +553,20 @@ def _attention_unfused(qkv: Split, att: Split, B: int, L: int, H: int, dh: int, 
     ops.gemm_raw(pa, va, o2, PASSES, 1)
 
 
+def attention(qkv: Split, att: Split, B: int, L: int, H: int, dh: int, D: int):
+    """att [B*L, D] = softmax(Q K^T / sqrt(dh)) V per (cloud, head) of qkv [B*L, 3D] (q | k | v), both split-bf16."""
+    if FUSED_ATTENTION and (dh == 64 or (dh == 88 and not ATTENTION_TWOPASS and FUSED_ATTENTION_DH88)) and (L <= 512 or FUSED_ATTENTION_LONG):
+        # fused wgmma attention: S and P stay in registers, key blocks stream through shared memory; V^T is read as an
+        # MN-major operand
+        mk = lambda col: qkv.operand(rows=L, k=dh, col=col, nb1=H, b1_stride=dh, nb2=B, b2_stride=L * qkv.pitch)
+        qa, ka, va = mk(0), mk(D), mk(2 * D)
+        entry = nv.lib().psam_attention_bf16x3_twopass if ATTENTION_TWOPASS else nv.lib().psam_attention_bf16x3
+        nv.check(entry(byref(qa), byref(ka), byref(va), att.ptr(), att.plane, att.pitch, dh, L * att.pitch, dh ** -0.5,
+                       nv.stream()), "attention_bf16x3")
+    else:
+        _attention_unfused(qkv, att, B, L, H, dh, D, qkv.t.device)
+
+
 def _run_block(pb: _PackedBlock, x: torch.Tensor, B: int, L: int, D: int, fold=None):
     """x fp32 [B*L, D], updated in place (pre-LN residual block, rope=None).
     fold = (xs, st_in, st_mid, st_out): LayerNorm-free form - xs is the split-bf16 copy of x and st_in its row statistics
@@ -538,16 +583,7 @@ def _run_block(pb: _PackedBlock, x: torch.Tensor, B: int, L: int, D: int, fold=N
         ops.layernorm(x, pb.g1, pb.b1, pb.eps1, out_split=xn)
         ops.gemm(xn, pb.wqkv, bias=pb.bqkv, out_split=qkv, passes=PASSES)
     att = Split(M, D, dev)
-    if FUSED_ATTENTION and (dh == 64 or (dh == 88 and not ATTENTION_TWOPASS and FUSED_ATTENTION_DH88)) and (L <= 512 or FUSED_ATTENTION_LONG):
-        # fused wgmma attention: S and P stay in registers, key blocks stream through shared memory; V^T is read as an
-        # MN-major operand
-        mk = lambda col: qkv.operand(rows=L, k=dh, col=col, nb1=H, b1_stride=dh, nb2=B, b2_stride=L * qkv.pitch)
-        qa, ka, va = mk(0), mk(D), mk(2 * D)
-        entry = nv.lib().psam_attention_bf16x3_twopass if ATTENTION_TWOPASS else nv.lib().psam_attention_bf16x3
-        nv.check(entry(byref(qa), byref(ka), byref(va), att.ptr(), att.plane, att.pitch, dh, L * att.pitch, dh ** -0.5,
-                       nv.stream()), "attention_bf16x3")
-    else:
-        _attention_unfused(qkv, att, B, L, H, dh, D, dev)
+    attention(qkv, att, B, L, H, dh, D)
     # x += proj(att)
     if fold is not None:
         # one writer per element (no split-K): the epilogue also emits split-bf16(x) and the row statistics for norm2

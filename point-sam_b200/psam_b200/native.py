@@ -74,6 +74,7 @@ EXPORTS = [
     "psam_nn_grid_workspace_bytes", "psam_nn_grid_f32", "psam_voxel_subsample_workspace_bytes", "psam_voxel_subsample_f32",
     "psam_mask_loss_stats", "psam_mask_loss_grad", "psam_interp_inverse", "psam_head_dp", "psam_head_dp_chunks",
     "psam_interp_ln_gelu_backward", "psam_interp_backward", "psam_sum_partials",
+    "psam_layernorm_backward", "psam_swiglu_ln_backward", "psam_gelu_backward", "psam_softmax_backward",
     "psam_version",
 ]
 
@@ -176,6 +177,10 @@ def lib():
             "psam_interp_ln_gelu_backward": [p, i, i, i, i, p, p, i, p, p, f, p, p, i, p],
             "psam_interp_backward": [p, i, i, i, i, p, p, p, i, p, p],
             "psam_sum_partials": [p, i, i, ll, p, p],
+            "psam_layernorm_backward": [p, ll, i, i, p, ll, p, f, p, ll, p, ll, p, ll, ll, p, i, p],
+            "psam_swiglu_ln_backward": [p, ll, i, i, i, p, ll, p, p, f, p, ll, p, ll, ll, p, ll, ll, p, i, p],
+            "psam_gelu_backward": [p, ll, i, i, p, ll, p, ll, p, ll, ll, p, ll, ll, p],
+            "psam_softmax_backward": [p, ll, p, ll, ll, i, f, p, ll, ll, p],
         }
         for name, args in sig.items():
             fn = getattr(L, name)

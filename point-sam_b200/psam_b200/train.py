@@ -140,7 +140,7 @@ def head_backward(f0, hyper, gamma, beta, w3, b3, geo, dm, need_f0=True, need_ln
         nv.check(nv.lib().psam_head_dp(nv.ptr(p), nv.ptr(dm[z0:z1]), nv.ptr(hyper[z0:z1]), nz, C, N, D, dps.ptr(), dps.plane,
                                        dps.pitch, nv.ptr(part_h[z0:z1]), nv.ptr(part_b[z0:z1]), nv.stream()), "head_dp")
         if need_w3:
-            part_w.append(_dw3_partials(dps, u1, R, D, dev))
+            part_w.append(_dw_partials(dps, u1, R))
         if need_du:
             du = p  # p is dead after head_dp: du1 = dp W3 overwrites it, and the LayerNorm backward turns it into dv in place
             ops.gemm(dps, w3t, out_f32=du, passes=engine.PASSES)
@@ -167,27 +167,39 @@ def head_backward(f0, hyper, gamma, beta, w3, b3, geo, dm, need_f0=True, need_ln
     return df0, dhyper, dgamma, dbeta, dw3, db3
 
 
-def _dw3_partials(dps: Split, u1: Split, R: int, D: int, dev) -> torch.Tensor:
-    """dW3 = dp^T u1 over the R rows of a chunk as S partial products [S, D, D] of DW_SPLIT_K rows each: both operands are
-    transposed to [D, R] (psam_transpose_split) and the K axis is cut into S batches of the split-bf16 GEMM (operand batch
-    dimension with a column stride), zero-padded to S * Kc columns."""
+def _dw_partials(dy: Split, x: Split, R: int) -> torch.Tensor:
+    """A weight gradient dW = dy^T x over R rows (dy [R, n], x [R, k]) as S partial products [S, n, k] of DW_SPLIT_K rows
+    each: both operands are transposed to [n | k, R] (psam_transpose_split) and the K axis is cut into S batches of the
+    split-bf16 GEMM (operand batch dimension with a column stride), zero-padded to S * Kc columns."""
+    n, k, dev = dy.cols, x.cols, dy.t.device
     S = max(1, -(-R // DW_SPLIT_K))
     Kc = ops._round_up(-(-R // S), 64)
     Kp = S * Kc
-    outs = torch.empty((S, D, D), dtype=torch.float32, device=dev)
+    outs = torch.empty((S, n, k), dtype=torch.float32, device=dev)
     ts = []
-    for src in (dps, u1):
-        t = Split(D, Kp, dev, pitch=Kp, zero=Kp != R)
-        nv.check(nv.lib().psam_transpose_split(src.ptr(), src.plane, src.pitch, 0, 0, t.ptr(), t.plane, t.pitch, 0, 0, R, D, 1, 1,
-                                               nv.stream()), "transpose_split")
+    for src in (dy, x):
+        t = Split(src.cols, Kp, dev, pitch=Kp, zero=Kp != R)
+        nv.check(nv.lib().psam_transpose_split(src.ptr(), src.plane, src.pitch, 0, 0, t.ptr(), t.plane, t.pitch, 0, 0, R, src.cols,
+                                               1, 1, nv.stream()), "transpose_split")
         ts.append(t)
-    a = ts[0].operand(rows=D, k=Kc, nb1=S, b1_stride=Kc)
-    w = ts[1].operand(rows=D, k=Kc, nb1=S, b1_stride=Kc)
+    a = ts[0].operand(rows=n, k=Kc, nb1=S, b1_stride=Kc)
+    w = ts[1].operand(rows=k, k=Kc, nb1=S, b1_stride=Kc)
     o = ops.GemmOut()
-    o.out_f32, o.ldo, o.out_b1 = nv.ptr(outs), D, D * D
+    o.out_f32, o.ldo, o.out_b1 = nv.ptr(outs), k, n * k
     o.alpha = 1.0
     ops.gemm_raw(a, w, o, engine.PASSES, 1)
     return outs
+
+
+def _weight_grad(dy: Split, x: Split, R: int) -> torch.Tensor:
+    """dW = dy^T x [n, k] over R rows, the partials finished in a fixed order."""
+    pw = _dw_partials(dy, x, R)
+    return _sum_partials(pw, 1, pw.shape[0], dy.cols * x.cols, torch.empty((dy.cols, x.cols), dtype=torch.float32, device=pw.device))
+
+
+def _col_sum(t: torch.Tensor) -> torch.Tensor:
+    """Column sums of t [R, n] fp32 (a bias gradient), sequential over the rows."""
+    return _sum_partials(t, 1, t.shape[0], t.shape[1], torch.empty(t.shape[1], dtype=torch.float32, device=t.device))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -319,3 +331,297 @@ def run_mask_decoder_train(md, pc_embeddings, pc_pe, sparse, dense, aux, multima
     geo = head_geometry(aux, G, Z // B, up[1].eps)
     masks = MaskHead.apply(f0, hyper, up[1].weight, up[1].bias, up[3].weight, up[3].bias, geo)
     return masks, iou_pred
+
+
+# ------------------------------------------------------------------------------------------------
+# the point-cloud encoder: EvaBlock backward recomputed from each block's input (pc_encoder.py:118-145)
+# ------------------------------------------------------------------------------------------------
+# most attention score rows (clouds x heads x L) one chunk of the block backward holds: six transient [rows, L] buffers of
+# 4 bytes per element, about 0.8 GB at the limit
+ATTENTION_SCORE_ELEMS = 1 << 25
+ENCODER_TRAINABLE = ("transformer.blocks.", "transformer.norm.", "transformer.fc_norm.", "out_proj.", "patch_proj.", "pos_embed.")
+
+
+def check_block_shape(blk, D: int):
+    """Refuses a trainable EvaBlock whose shapes the backward has no kernel for (NotImplementedError, before any device
+    work): its split-bf16 operands start at column offsets h * dh, D and 2 D, which the GEMM needs 16-byte aligned."""
+    H = blk.attn.num_heads
+    if D % H or D % 8 or (D // H) % 8:
+        raise NotImplementedError(f"encoder fine-tuning supports blocks whose width and head dim are multiples of 8, got width {D} "
+                                  f"with {H} heads")
+
+
+class _SplitRows(Split):
+    """Rows [r0, r0 + n) of a split-bf16 matrix, sharing its storage (the lo plane stays one full plane after the hi)."""
+    __slots__ = ("_plane",)
+
+    def __init__(self, s: Split, r0: int, n: int):
+        self.t, self.rows, self.cols, self.pitch, self._plane = s.t[:, r0:r0 + n], n, s.cols, s.pitch, s.plane
+
+    @property
+    def plane(self) -> int:
+        return self._plane
+
+
+def _transposes(pb, blk):
+    """W^T operands of the block's dX products, packed on the first backward and kept with the block's pack."""
+    if pb.transposed is None:
+        D = pb.D
+        mlp = blk.mlp
+        wqkv, _ = engine.qkv_weights(blk.attn, D)
+        if pb.swiglu:
+            w1 = engine.swiglu_fc1(mlp, pb.hp)[0]
+            w2 = engine.swiglu_fc2(mlp, pb.hp)
+        else:
+            w1, w2 = mlp.fc1.weight.detach().float(), mlp.fc2.weight.detach().float()
+        pack_t = lambda w: ops.pack_weight(w.t())
+        pb.transposed = types.SimpleNamespace(wqkv=pack_t(wqkv), wproj=pack_t(blk.attn.proj.weight.detach().float()), w1=pack_t(w1),
+                                              w2=pack_t(w2))
+    return pb.transposed
+
+
+def _ln_backward(x, dy, gamma, eps, dres=None, out_split=None):
+    """(dx [M, D], part [blocks, 2, D]) of a LayerNorm over the rows of x (psam_layernorm_backward)."""
+    M, D = x.shape
+    dx = torch.empty_like(x)
+    nblk = (M + LN_ROWS_PER_BLOCK - 1) // LN_ROWS_PER_BLOCK
+    part = torch.empty((nblk, 2, D), dtype=torch.float32, device=x.device)
+    nv.check(nv.lib().psam_layernorm_backward(nv.ptr(x), D, M, D, nv.ptr(dy), dy.shape[1], nv.ptr(gamma), float(eps), nv.ptr(dres), D,
+                                              nv.ptr(dx), D, out_split.ptr() if out_split is not None else None,
+                                              out_split.plane if out_split is not None else 0,
+                                              out_split.pitch if out_split is not None else 0, nv.ptr(part), LN_ROWS_PER_BLOCK,
+                                              nv.stream()), "layernorm_backward")
+    return dx, part
+
+
+def _ln_params(part):
+    nblk, _, D = part.shape
+    gb = _sum_partials(part, 1, nblk, 2 * D, torch.empty((2, D), dtype=torch.float32, device=part.device))
+    return gb[0], gb[1]
+
+
+def _attention_backward(qkv: Split, datt: Split, dqkv: torch.Tensor, B: int, L: int, H: int, dh: int, D: int):
+    """dqkv [B*L, 3D] fp32 (dQ | dK | dV) from datt = dL/d(attention output), per (cloud, head) through the GEMM's batch
+    dimensions: S = Q K^T recomputed, dP = dO V^T, dS = scale P (dP - rowsum(dP P)), dQ = dS K, dK = dS^T Q, dV = P^T dO.
+    Clouds are processed in chunks of at most ATTENTION_SCORE_ELEMS score elements."""
+    dev = dqkv.device
+    Lp = ops._round_up(L, 64)
+    scale = dh ** -0.5
+    cpc = max(1, ATTENTION_SCORE_ELEMS // (H * L * Lp))
+    for c0 in range(0, B, cpc):
+        nb = min(cpc, B - c0)
+        q, dO = _SplitRows(qkv, c0 * L, nb * L), _SplitRows(datt, c0 * L, nb * L)
+        rows = nb * H * L
+
+        def heads_t(src, col):  # [nb, H, dh, Lp]: the per-head column block of src transposed
+            t = Split(nb * H * dh, L, dev, pitch=Lp, zero=Lp != L)
+            nv.check(nv.lib().psam_transpose_split(src.ptr(col), src.plane, src.pitch, dh, L * src.pitch, t.ptr(), t.plane, t.pitch,
+                                                   dh * Lp, H * dh * Lp, L, dh, H, nb, nv.stream()), "transpose_split")
+            return t.operand(rows=dh, k=L, nb1=H, b1_stride=dh * Lp, nb2=nb, b2_stride=H * dh * Lp)
+
+        def heads(src, col):  # per-head [L, dh] blocks of src
+            return src.operand(rows=L, k=dh, col=col, nb1=H, b1_stride=dh, nb2=nb, b2_stride=L * src.pitch)
+
+        def square(t: Split):  # per-head [L, L] blocks
+            return t.operand(rows=L, k=L, nb1=H, b1_stride=L * Lp, nb2=nb, b2_stride=H * L * Lp)
+
+        def scores(a, w):
+            out = torch.empty((rows, L), dtype=torch.float32, device=dev)
+            o = ops.GemmOut()
+            o.out_f32, o.ldo, o.out_b1, o.out_b2 = nv.ptr(out), L, L * L, H * L * L
+            o.alpha = 1.0
+            ops.gemm_raw(a, w, o, engine.PASSES, 1)
+            return out
+
+        def into_dqkv(a, w, col):
+            o = ops.GemmOut()
+            o.out_f32, o.ldo, o.out_b1, o.out_b2 = nv.ptr(dqkv) + 4 * (c0 * L * 3 * D + col), 3 * D, dh, L * 3 * D
+            o.alpha = 1.0
+            ops.gemm_raw(a, w, o, engine.PASSES, 1)
+
+        s = scores(heads(q, 0), heads(q, D))
+        dp = scores(heads(dO, 0), heads(q, 2 * D))
+        ds = Split(rows, L, dev, pitch=Lp, zero=Lp != L)
+        nv.check(nv.lib().psam_softmax_backward(nv.ptr(s), L, nv.ptr(dp), L, rows, L, scale, ds.ptr(), ds.plane, ds.pitch, nv.stream()),
+                 "softmax_backward")
+        del dp
+        p = Split(rows, L, dev, pitch=Lp, zero=Lp != L)
+        ops.softmax_split(s, L, scale, p)
+        del s
+
+        def square_t(src: Split):
+            t = Split(rows, L, dev, pitch=Lp, zero=Lp != L)
+            nv.check(nv.lib().psam_transpose_split(src.ptr(), src.plane, src.pitch, L * Lp, H * L * Lp, t.ptr(), t.plane, t.pitch,
+                                                   L * Lp, H * L * Lp, L, L, H, nb, nv.stream()), "transpose_split")
+            return t
+
+        into_dqkv(square(ds), heads_t(q, D), 0)                    # dQ = dS K
+        into_dqkv(square(square_t(ds)), heads_t(q, 0), D)          # dK = dS^T Q
+        del ds
+        into_dqkv(square(square_t(p)), heads_t(dO, 0), 2 * D)      # dV = P^T dO
+        del p
+
+
+def block_backward(blk, pb, x: torch.Tensor, dy: torch.Tensor, B: int, L: int, need_x: bool = True):
+    """Gradients of one EvaBlock (pre-LN attention + SwiGLU / GELU MLP, rope=None) at its input x [B*L, D] fp32 for the
+    upstream gradient dy [B*L, D]: (dx or None, {parameter name: gradient}).  The forward is recomputed from x (unfused
+    LayerNorms), keeping what one block needs; dx = None when need_x is false and norm1 is frozen."""
+    D, H, dh = pb.D, pb.H, pb.dh
+    M = B * L
+    dev = x.device
+    tr = _transposes(pb, blk)
+    # ---- forward, recomputed
+    xn = Split(M, D, dev)
+    ops.layernorm(x, pb.g1, pb.b1, pb.eps1, out_split=xn)
+    qkv = Split(M, 3 * D, dev)
+    ops.gemm(xn, pb.wqkv, bias=pb.bqkv, out_split=qkv, passes=engine.PASSES)
+    att = Split(M, D, dev)
+    engine.attention(qkv, att, B, L, H, dh, D)
+    x1 = x.clone()
+    ops.gemm(att, pb.wproj, bias=pb.bproj, out_f32=x1, resid=x1, passes=engine.PASSES)
+    xn2 = Split(M, D, dev)
+    ops.layernorm(x1, pb.g2, pb.b2, pb.eps2, out_split=xn2)
+    n1 = 2 * pb.hp if pb.swiglu else pb.hid
+    a = torch.empty((M, n1), dtype=torch.float32, device=dev)
+    ops.gemm(xn2, pb.w1, bias=pb.bb1, out_f32=a, passes=engine.PASSES)
+    # ---- MLP
+    g = {}
+    dys = Split(M, D, dev)
+    ops.split_f32(dy, dys)
+    das = Split(M, n1, dev)
+    mlp = blk.mlp
+    if pb.swiglu:
+        Hd, Hp = pb.hid, pb.hp
+        dhn = torch.empty((M, Hp), dtype=torch.float32, device=dev)
+        ops.gemm(dys, tr.w2, out_f32=dhn, passes=engine.PASSES)
+        hn = Split(M, Hp, dev, pitch=Hp)
+        da = torch.empty_like(a)
+        nblk = (M + LN_ROWS_PER_BLOCK - 1) // LN_ROWS_PER_BLOCK
+        part = torch.empty((nblk, 2, Hd), dtype=torch.float32, device=dev)
+        nv.check(nv.lib().psam_swiglu_ln_backward(nv.ptr(a), n1, M, Hd, Hp, nv.ptr(dhn), Hp, nv.ptr(pb.gn), nv.ptr(pb.bn), float(pb.epsn),
+                                                  nv.ptr(da), n1, das.ptr(), das.plane, das.pitch, hn.ptr(), hn.plane, hn.pitch, nv.ptr(part),
+                                                  LN_ROWS_PER_BLOCK, nv.stream()), "swiglu_ln_backward")
+        del dhn
+        g["mlp.norm.weight"], g["mlp.norm.bias"] = _ln_params(part)
+        g["mlp.fc2.weight"] = _weight_grad(dys, hn, M)[:, :Hd]
+        del hn
+        db1 = _col_sum(da)
+        dw1 = _weight_grad(das, xn2, M)
+        g["mlp.fc1_g.weight"], g["mlp.fc1_x.weight"] = dw1[0:2 * Hd:2], dw1[1:2 * Hd:2]
+        g["mlp.fc1_g.bias"], g["mlp.fc1_x.bias"] = db1[0:2 * Hd:2], db1[1:2 * Hd:2]
+    else:
+        dh_ = torch.empty((M, n1), dtype=torch.float32, device=dev)
+        ops.gemm(dys, tr.w2, out_f32=dh_, passes=engine.PASSES)
+        h = Split(M, n1, dev)
+        da = a  # the GELU backward reads a[i] before it writes da[i]
+        nv.check(nv.lib().psam_gelu_backward(nv.ptr(a), n1, M, n1, nv.ptr(dh_), n1, nv.ptr(da), n1, das.ptr(), das.plane, das.pitch,
+                                             h.ptr(), h.plane, h.pitch, nv.stream()), "gelu_backward")
+        del dh_
+        g["mlp.fc2.weight"] = _weight_grad(dys, h, M)
+        del h
+        g["mlp.fc1.bias"] = _col_sum(da)
+        g["mlp.fc1.weight"] = _weight_grad(das, xn2, M)
+    g["mlp.fc2.bias"] = _col_sum(dy)
+    del da, a
+    dxn2 = torch.empty((M, D), dtype=torch.float32, device=dev)
+    ops.gemm(das, tr.w1, out_f32=dxn2, passes=engine.PASSES)
+    del das
+    dx1s = Split(M, D, dev)
+    dx1, part2 = _ln_backward(x1, dxn2, pb.g2, pb.eps2, dres=dy, out_split=dx1s)
+    del dxn2, x1
+    g["norm2.weight"], g["norm2.bias"] = _ln_params(part2)
+    # ---- attention
+    g["attn.proj.weight"] = _weight_grad(dx1s, att, M)
+    g["attn.proj.bias"] = _col_sum(dx1)
+    datt = Split(M, D, dev)
+    ops.gemm(dx1s, tr.wproj, out_split=datt, passes=engine.PASSES)
+    del dx1s, att
+    dqkv = torch.empty((M, 3 * D), dtype=torch.float32, device=dev)
+    _attention_backward(qkv, datt, dqkv, B, L, H, dh, D)
+    del qkv, datt
+    dqkvs = Split(M, 3 * D, dev)
+    ops.split_f32(dqkv, dqkvs)
+    dwqkv, dbqkv = _weight_grad(dqkvs, xn, M), _col_sum(dqkv)
+    del dqkv
+    at = blk.attn
+    if getattr(at, "qkv", None) is not None:
+        g["attn.qkv.weight"], g["attn.q_bias"], g["attn.v_bias"] = dwqkv, dbqkv[:D], dbqkv[2 * D:]
+    else:
+        for i, n in enumerate(("q_proj", "k_proj", "v_proj")):
+            g[f"attn.{n}.weight"], g[f"attn.{n}.bias"] = dwqkv[i * D:(i + 1) * D], dbqkv[i * D:(i + 1) * D]
+    dx = None
+    if need_x or blk.norm1.weight.requires_grad or blk.norm1.bias.requires_grad:
+        dxn = torch.empty((M, D), dtype=torch.float32, device=dev)
+        ops.gemm(dqkvs, tr.wqkv, out_f32=dxn, passes=engine.PASSES)
+        dx, part1 = _ln_backward(x, dxn, pb.g1, pb.eps1, dres=dx1)
+        g["norm1.weight"], g["norm1.bias"] = _ln_params(part1)
+    return (dx if need_x else None), g
+
+
+class EvaBlockFn(torch.autograd.Function):
+    """One EvaBlock as an autograd node: the forward is the engine's inference block (un-folded LayerNorms) on a copy of
+    x [B*L, D]; the inputs after the block's pack are its live parameters (named_parameters order), so their gradients land
+    on the module.  Saves x only; the backward (block_backward) recomputes the rest."""
+
+    @staticmethod
+    def forward(ctx, x, blk, pb, B, L, *params):
+        y = x.detach().clone()
+        engine._run_block(pb, y, B, L, pb.D)
+        ctx.save_for_backward(x)
+        ctx.blk, ctx.pb, ctx.B, ctx.L = blk, pb, B, L
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        dx, g = block_backward(ctx.blk, ctx.pb, x.detach(), dy.float().contiguous(), ctx.B, ctx.L, need_x=need[0])
+        names = [n for n, _ in ctx.blk.named_parameters()]
+        return (dx, None, None, None, None) + tuple(g[n].contiguous() if need[5 + i] else None for i, n in enumerate(names))
+
+
+def encoder_trains(enc) -> bool:
+    return any(p.requires_grad for p in enc.parameters())
+
+
+def run_pc_encoder_train(enc, coords, features):
+    """PointCloudEncoder.forward with autograd into the trainable parameters of the transformer blocks, the tail LayerNorms,
+    out_proj, patch_proj and pos_embed: returns (pc_embeddings [B, L, E] with grad_fn, patches).  The tokenizer and the
+    blocks below the lowest trainable one run through the engine without gradient; every block from there on is an
+    EvaBlockFn; patch_proj / pos_embed (when trainable), the tail and out_proj are torch autograd on the per-token rows."""
+    if hasattr(enc.patch_embed, "grouper1"):
+        raise NotImplementedError("encoder fine-tuning covers the kNN tokenizer (PatchEmbed); PatchEmbedHier is not implemented")
+    pk = engine._cached(enc, engine._PackedEncoder)
+    tail = engine.validate_transformer(enc.transformer)
+    blocks = list(enc.transformer.blocks)
+    D = enc.transformer_dim
+    with torch.no_grad():
+        patches = engine.run_knn_grouper(enc.patch_embed.grouper, coords, features)
+        emb, embs = engine.run_patch_encoder(enc.patch_embed.patch_encoder, patches["features"], want_split=True)
+        patches["embeddings"] = emb
+    B, L, _ = emb.shape
+    M, dev = B * L, emb.device
+    centers = patches["centers"]
+    trains = lambda m: any(p.requires_grad for p in m.parameters())
+    if trains(enc.patch_proj) or trains(enc.pos_embed):
+        pe = enc.pos_embed
+        x = _linear(enc.patch_proj, emb) + _linear(pe[2], F.gelu(_linear(pe[0], centers)))
+        x = x.reshape(M, D)
+        lo = 0
+    else:
+        with torch.no_grad():
+            x = torch.empty((M, D), dtype=torch.float32, device=dev)
+            ops.gemm(embs, pk.wpp, bias=pk.bpp, out_f32=x, passes=engine.PASSES)
+            pos = Split(M, pk.wpos0.shape[0], dev)
+            ops.small_in_linear(centers, pk.wpos0, pk.bpos0, None, None, 0.0, False, ops.ACT_GELU, pos)
+            ops.gemm(pos, pk.wpos2, bias=pk.bpos2, out_f32=x, resid=x, passes=engine.PASSES)
+        lo = next((i for i, b in enumerate(blocks) if trains(b)), len(blocks))
+    with torch.no_grad():
+        for pb in pk.blocks[:lo]:
+            engine._run_block(pb, x, B, L, D)
+    for blk, pb in zip(blocks[lo:], pk.blocks[lo:]):
+        x = EvaBlockFn.apply(x, blk, pb, B, L, *blk.parameters())
+    for m in tail:
+        x = _ln(m, x)
+    out = _linear(enc.out_proj, x).reshape(B, L, -1)
+    return out, patches
